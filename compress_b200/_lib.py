@@ -87,6 +87,9 @@ def _load():
     lib.b2c_decode_profile_read.argtypes = [c.c_void_p, c.c_void_p]
     lib.b2c_decode_staged_count.restype = c.c_int
     lib.b2c_decode_staged_count.argtypes = [c.c_void_p, c.c_uint32, c.c_void_p]
+    for nm in ("b2c_decode_staged_flags", "b2c_s2_decode_staged_flags"):
+        getattr(lib, nm).restype = c.c_int
+        getattr(lib, nm).argtypes = [c.c_void_p, c.c_uint32, c.c_void_p]
     lib.b2c_zstd_decode_device.restype = c.c_int
     lib.b2c_zstd_decode_device.argtypes = [
         c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_uint32,
@@ -145,6 +148,7 @@ EXPORTED_SYMBOLS = [
     "b2c_sm_count", "b2c_launch_count", "b2c_zstd_bound", "b2c_zstd_encode_device",
     "b2c_zstd_encode_chunks", "b2c_zstd_encode_device_debug", "b2c_zstd_encode_packed", "b2c_zstd_encode_device_timed",
     "b2c_zstd_decode_device", "b2c_zstd_decode_chunks", "b2c_profile_enable", "b2c_profile_read", "b2c_decode_profile_enable", "b2c_decode_profile_read", "b2c_decode_staged_count", "b2c_s2_decode_staged_count",
+    "b2c_decode_staged_flags", "b2c_s2_decode_staged_flags",
     "b2c_huf_compress_device", "b2c_huf_decompress_device",
     "b2c_s2_bound", "b2c_s2_encode_device", "b2c_s2_decode_device", "b2c_s2_encode_chunks", "b2c_s2_decode_chunks",
     "b2c_huf_compress_chunks", "b2c_huf_decompress_chunks", "b2c_huf_read_table",

@@ -79,6 +79,7 @@ struct b2c_ctx {
     uint8_t *d_fd_seq = nullptr; size_t fd_seq_cap = 0;    //   sequence records
     uint8_t *d_fd_lit = nullptr; size_t fd_lit_cap = 0;    //   decoded literals
     int dec_staged = 1;                                    // B2C_DEC=onewarp: one-warp decoder only (A/B measurements)
+    bool fd_last = false, s2d_last = false;                // the most recent zstd / S2 decode launch ran the staged kernels
     float dec_ms[6] = {0, 0, 0, 0, 0, 0}; cudaEvent_t dec_ev[7] = {}; int dec_prof = 0;
     uint8_t *d_dec_in = nullptr, *d_dec_out = nullptr; size_t dec_in_cap = 0, dec_out_cap = 0;
     uint8_t *d_dec_meta = nullptr; size_t dec_meta_cap = 0;
@@ -372,36 +373,46 @@ int b2c_decode_profile_enable(b2c_ctx *ctx, int on) {
     for (int i = 0; i < 6; i++) ctx->dec_ms[i] = 0.f;
     return B2C_OK;
 }
-// How many of the first nchunks inputs of the most recent decode launch were completed by the staged kernels (the others
-// went through the one-warp decoder).  Synchronises the device.  Test / diagnostics hook.
-int b2c_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
-    if (!ctx || !staged) return B2C_ERR_ARG;
-    *staged = 0;
-    if (!ctx->d_fd || !ctx->dec_staged || nchunks == 0) return B2C_OK;
+// flags[i] = 1 where the per-input record (whose first word is its state; 0 = finished by the staged kernels) says so.
+// last: the most recent launch ran the staged kernels (otherwise the records are an earlier launch's and every flag is 0).
+static int staged_flags(b2c_ctx *ctx, const uint8_t *recs, bool last, size_t rec_bytes, size_t cap, uint32_t nchunks, uint8_t *flags) {
+    memset(flags, 0, nchunks);
+    if (!recs || !last || nchunks == 0) return B2C_OK;
     CK(cudaSetDevice(ctx->device));
     CK(cudaDeviceSynchronize());
-    if ((size_t)nchunks * sizeof(FdChunk) > ctx->fd_cap) return B2C_ERR_ARG;
+    if ((size_t)nchunks * rec_bytes > cap) return B2C_ERR_ARG;
     std::vector<uint32_t> st(nchunks);
-    CK(cudaMemcpy2D(st.data(), sizeof(uint32_t), ctx->d_fd, sizeof(FdChunk), sizeof(uint32_t), nchunks, cudaMemcpyDeviceToHost));
-    uint32_t k = 0;
-    for (uint32_t v : st) k += v == 0;
-    *staged = k;
+    CK(cudaMemcpy2D(st.data(), sizeof(uint32_t), recs, rec_bytes, sizeof(uint32_t), nchunks, cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < nchunks; i++) flags[i] = st[i] == 0;
     return B2C_OK;
 }
+// Per input of the first nchunks of the most recent decode launch: 1 if the staged kernels completed it, 0 if it went
+// through the one-warp decoder.  Synchronises the device.  Test / diagnostics hook.
+int b2c_decode_staged_flags(b2c_ctx *ctx, uint32_t nchunks, uint8_t *flags) {
+    if (!ctx || (!flags && nchunks)) return B2C_ERR_ARG;
+    return staged_flags(ctx, ctx->d_fd, ctx->fd_last, sizeof(FdChunk), ctx->fd_cap, nchunks, flags);
+}
 // The same for the most recent S2 block decode launch: blocks finished by the staged kernels (tag walk + execution).
+int b2c_s2_decode_staged_flags(b2c_ctx *ctx, uint32_t nchunks, uint8_t *flags) {
+    if (!ctx || (!flags && nchunks)) return B2C_ERR_ARG;
+    return staged_flags(ctx, ctx->d_s2d, ctx->s2d_last, sizeof(S2Head), ctx->s2d_cap, nchunks, flags);
+}
+// How many of the first nchunks inputs of the most recent decode launch the staged kernels completed.
+int b2c_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
+    if (!ctx || !staged) return B2C_ERR_ARG;
+    std::vector<uint8_t> f(nchunks);
+    const int rc = b2c_decode_staged_flags(ctx, nchunks, f.data());
+    *staged = 0;
+    for (uint8_t v : f) *staged += v;
+    return rc;
+}
 int b2c_s2_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
     if (!ctx || !staged) return B2C_ERR_ARG;
+    std::vector<uint8_t> f(nchunks);
+    const int rc = b2c_s2_decode_staged_flags(ctx, nchunks, f.data());
     *staged = 0;
-    if (!ctx->d_s2d || !ctx->dec_staged || nchunks == 0) return B2C_OK;
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaDeviceSynchronize());
-    if ((size_t)nchunks * sizeof(S2Head) > ctx->s2d_cap) return B2C_ERR_ARG;
-    std::vector<uint32_t> st(nchunks);
-    CK(cudaMemcpy2D(st.data(), sizeof(uint32_t), ctx->d_s2d, sizeof(S2Head), sizeof(uint32_t), nchunks, cudaMemcpyDeviceToHost));
-    uint32_t k = 0;
-    for (uint32_t v : st) k += v == 0;
-    *staged = k;
-    return B2C_OK;
+    for (uint8_t v : f) *staged += v;
+    return rc;
 }
 int b2c_decode_profile_read(b2c_ctx *ctx, double *ms) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
@@ -1070,6 +1081,7 @@ static int launch_decode(b2c_ctx *ctx, ZstdDecParams &P, cudaStream_t st, uint64
     if (n <= 4096) { maxb = (uint32_t)(65536 / n); if (maxb > FD_MAXB_LONG) maxb = FD_MAXB_LONG; }      // (>= 16 blocks per input)
     const bool perBlock = maxb > FD_MAXB;
     const bool staged = ctx->dec_staged && lit_span > 0 && lit_span <= kStagedSpanLimit && (uint64_t)n * maxb * FD_TAB_ENTRIES < (1ull << 31);
+    ctx->fd_last = staged;
     if (staged) {
         const size_t recBytes = (((size_t)n * sizeof(FdChunk)) + 255) & ~(size_t)255;
         const size_t blkBytes = (((size_t)n * maxb * sizeof(FdBlock)) + 255) & ~(size_t)255;
@@ -1566,7 +1578,10 @@ int b2c_s2_decode_stream(b2c_ctx *ctx, const void *src, size_t n, void *dst, siz
 // block); the one-warp kernel then takes what they left (large or unusual blocks, errors).
 static int launch_s2_decode(b2c_ctx *ctx, S2DecParams &P, uint64_t span, cudaStream_t st) {
     const uint32_t n = P.nchunks;
+    // (a call with per-block source offsets passes span 0: the element records are placed by the offsets, whose extent the
+    // host does not know, so such a call runs the one-warp kernel alone)
     const bool staged = ctx->dec_staged && span > 0 && span <= ((uint64_t)8 << 30);
+    ctx->s2d_last = staged;
     if (staged) {
         const size_t headBytes = (((size_t)n * sizeof(S2Head)) + 255) & ~(size_t)255;
         const size_t recBytes = ((size_t)(span / 3) + n + 16) * sizeof(uint64_t);

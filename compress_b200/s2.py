@@ -145,6 +145,12 @@ class Codec:
         check(lib.b2c_s2_decode_staged_count(self._ctx, n, ctypes.byref(k)), self._ctx)
         return int(k.value)
 
+    def staged_flags(self, n):
+        """Per block of the first n of the last decode launch: 1 if the staged kernels finished it, else 0 (uint8 ndarray)."""
+        f = np.zeros(n, dtype=np.uint8)
+        check(lib.b2c_s2_decode_staged_flags(self._ctx, n, f.ctypes.data), self._ctx)
+        return f
+
     def _host(self, fn, blobs, caps, *pre):
         n = len(blobs)
         bufs = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(0, dtype=np.uint8) for b in blobs]

@@ -363,6 +363,13 @@ class Decoder:
         check(lib.b2c_decode_staged_count(self._ctx, n, ctypes.byref(k)), self._ctx)
         return int(k.value)
 
+    def staged_flags(self, n):
+        """Per input of the first n of the most recent decode launch: 1 if the staged kernels completed it, else 0 (uint8
+        ndarray)."""
+        f = np.zeros(n, dtype=np.uint8)
+        check(lib.b2c_decode_staged_flags(self._ctx, n, f.ctypes.data), self._ctx)
+        return f
+
     def decode_device(self, src, src_sizes, src_offsets=None, src_stride=0, dst=None, dst_cap=CHUNK, dst_offsets=None,
                       out_sizes=None, dst_stride=None):
         """src: uint8 CUDA tensor; stream i is src[off_i : off_i + src_sizes[i]] with off_i = src_offsets[i]
