@@ -227,6 +227,9 @@ b2c_ctx *b2c_ctx_create(int device, size_t max_chunks) {
     ok = ok && cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(b2c_zstd_chains_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)CHAIN_SMEM_BYTES) == cudaSuccess;
+    // at most two chains CTAs per SM, the rest of the SM's memory stays L1: a 16384-chunk pass (512 CTAs) took
+    // 1.21 ms per GiB with four CTAs sharing an SM and 0.99 ms with two (H100 SXM at 700 W, level 1)
+    ok = ok && cudaFuncSetAttribute(b2c_zstd_chains_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 50) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(b2c_huf_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)HUF0_SMEM_BYTES) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(b2c_huf_decompress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -471,7 +474,10 @@ static int launch_encode(b2c_ctx *ctx, int level, int flags, const void *d_src, 
     CK(cudaSetDevice(ctx->device));
     const uint32_t blockmax = level_block(level);
     const uint64_t pstride = wk_pool_stride(blockmax);
-    const uint32_t subMax = blockmax > 65536 ? 4096u : 8192u;   // work pool: 2.8 GB (64 KiB blocks) / 3.4 GB (128 KiB blocks)
+    // One pass takes a 1 GiB batch (16384 x 64 KiB or 8192 x 128 KiB) in one go: every kernel's drain and tail is paid
+    // once, and the persistent parse and the chains kernel have enough chunks to fill the device.  Work pool: 345 KB per
+    // 64 KiB chunk (5.7 GB at 16384), 821 KB per 128 KiB block (6.7 GB at 8192); it grows only for calls that large.
+    const uint32_t subMax = blockmax > 65536 ? 8192u : 16384u;
     const uint32_t sub = nchunks < subMax ? nchunks : subMax;
     if (ctx->work_cap[slot] < sub || ctx->pool_cap[slot] < (size_t)sub * pstride) {
         // grow the per-chunk work records / pool (kernels of earlier calls on other streams may still use the old ones)

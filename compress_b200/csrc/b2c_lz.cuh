@@ -12,14 +12,15 @@
 // output, on HTML -12 %.  A fully dynamic table is serial; what is built here is the parallel form that keeps most of
 // it: positions are inserted in TILES (4 per thread, in position order); a slot holds the earliest position of the
 // latest tile that touched it.  A position therefore sees (a) "far": the slot as the earlier tiles left it and (b) "near":
-// the earliest equal-hash position of its own tile, when that lies before it.  Per tile: probe (far) | barrier | plain
-// stores | barrier | losers of a store race fix the slot with atomicMin (exact minimum, so the result never depends
-// on scheduling) | barrier | probe (near).  Slots are 32-bit: position << 14 | 14 hash bits, so a candidate is
-// accepted by its tag and the dense pass never reads the input at the candidate (random shared-memory reads are what
-// bounded the round-1 kernel: about 3.4 bank-conflict cycles per warp access, five accesses per position there, four
-// here for a much better parse).  The chunk itself is streamed from global memory during the dense pass (coalesced,
-// prefetched one tile ahead) and only afterwards staged into the dead table's shared memory by one TMA bulk copy for
-// the random accesses of the walk.
+// the earliest equal-hash position of its own tile, when that lies before it.  Per tile: probe (far) | barrier | one
+// atomicMax per inserted position | barrier | probe (near).  Slots are 32-bit keys, tile-major (tile, then the
+// position's distance from the tile's end, then 14 hash bits: see LZ_KEYX), so the largest key is the earliest position
+// of the latest tile and the result never depends on scheduling.  A key decodes to position << 14 | tag with one XOR,
+// so a candidate is accepted by its tag and the dense pass never reads the input at the candidate (random shared-memory
+// reads are what bounded the round-1 kernel: about 3.4 bank-conflict cycles per warp access, five accesses per
+// position there, three here for a much better parse).  The chunk itself is streamed from global memory during the
+// dense pass (coalesced, prefetched one tile ahead) and only afterwards staged into the dead table's shared memory by
+// one TMA bulk copy for the random accesses of the walk.
 //
 // After the dense pass every thread runs the greedy scan over its own 128-byte range (set bit -> candidate distance
 // from a per-CTA scratch array -> extend forwards/backwards -> emit -> skip), neighbours are merged by a prefix
@@ -36,7 +37,13 @@ constexpr uint32_t LZ_RANGE = 128;          // bytes walked by one thread
 constexpr uint32_t LZ_MAXREC = LZ_RANGE / 4;   // matches a thread can start inside its range (min match 4)
 constexpr uint32_t LZ_TAGBITS = 14;
 constexpr uint32_t LZ_TAGMASK = (1u << LZ_TAGBITS) - 1;
-constexpr uint32_t LZ_EMPTY = 0xffffffffu;
+// A table slot holds a KEY: the entry (position << 14 | tag) XOR LZ_KEYX<TILE>.  Flipping the position's low log2(TILE)
+// bits makes it (tile << log2 TILE) | (TILE - 1 - position in tile), so atomicMax keeps the earliest position of the
+// latest tile; bit 31 (positions are < 2^17, so entries use 31 bits) sets every key above LZ_EMPTY = ~LZ_KEYX, which
+// therefore loses every atomicMax and decodes to the all-ones entry, the empty slot of the store / atomicMin protocol
+// this replaced (same table contents, same candidates, same output).
+template <uint32_t TILE> constexpr uint32_t LZ_KEYX = 0x80000000u | ((TILE - 1) << 14);
+template <uint32_t TILE> constexpr uint32_t LZ_EMPTY = ~LZ_KEYX<TILE>;
 #ifndef LZ_PPT1
 #define LZ_PPT1 8           // positions per thread and tile of the single-table configurations (4 or 8)
 #endif
@@ -179,18 +186,21 @@ B2C_DEV uint32_t lz_rec_d(uint32_t r) { return r >> 16; }
 
 // One tile of the dense pass for the four positions 4g .. 4g+3 of this thread (words w0..w2 hold their 11 bytes).
 // GUARD: the tile reaches past the last hashable position (only the last tile of a chunk).
-// A slot is position << 14 | tag, so for a slot r and this position's entry e the difference t = e - r is
-// (distance << 14) exactly when the tags agree and r lies before e: "t & (sign | tag bits) == 0" is the whole
-// acceptance test and t >> 14 the candidate's distance (an empty slot, all ones, can only pass with a distance beyond
-// the position, which the walk rejects).
+// A slot decodes (key ^ KX) to an entry r = position << 14 | tag, so for this position's entry e the difference t = e - r
+// is (distance << 14) exactly when the tags agree and r lies before e: "t & (sign | tag bits) == 0" is the whole
+// acceptance test and t >> 14 the candidate's distance (an empty slot decodes to all ones and can only pass with a
+// distance beyond the position, which the walk rejects).
 template <int LV, bool GUARD>
 B2C_DEV void lz_dense_tile(uint32_t *TS, uint32_t *TL, uint32_t *bm, uint32_t *bml, uint16_t *cd, uint32_t g, uint32_t npos,
                            const uint32_t (&wv)[LzCfg<LV>::PPT < 4 ? 3 : LzCfg<LV>::PPT / 4 + 2], unsigned lane) {
     using C = LzCfg<LV>;
     constexpr int PPT = C::PPT;
     constexpr uint32_t BAD = 0x80000000u | LZ_TAGMASK | (C::BLOCK > 65536 ? 0x40000000u : 0u);   // wrong tag, not earlier, or >= 64 KiB away
+    constexpr uint32_t KX = LZ_KEYX<C::NT * C::PPT>;
+    static_assert(C::BLOCK <= (1u << 17) && ((C::NT * C::PPT) & (C::NT * C::PPT - 1)) == 0,
+                  "keys need positions below 2^17 and tiles of a power-of-two size");
     const uint32_t p0 = PPT * g;
-    uint32_t hs[PPT], fs[PPT];                  // short table: hash (index = high bits, tag = low bits) and far slot content
+    uint32_t hs[PPT], fs[PPT];                  // short table: hash (index = high bits, tag = low bits) and far slot entry
     uint32_t hl[C::LONG ? PPT : 1], fl[C::LONG ? PPT : 1];
 #define LZ_IDX(h) ((h) >> (32 - C::TBITS))
 #define LZ_ENT(h, j) (((p0 + (j)) << LZ_TAGBITS) | ((h) & LZ_TAGMASK))
@@ -208,37 +218,20 @@ B2C_DEV void lz_dense_tile(uint32_t *TS, uint32_t *TL, uint32_t *bm, uint32_t *b
             hi = (j & 3) ? __funnelshift_r(bb, c, 8 * (j & 3)) : bb;
         }
         hs[j] = lz_hash_short<C::SMLS>(lo, hi);
-        fs[j] = TS[LZ_IDX(hs[j])];                                     // far candidate: the slot as earlier tiles left it
+        fs[j] = TS[LZ_IDX(hs[j])] ^ KX;                                // far candidate: the slot as earlier tiles left it
         if constexpr (C::LONG) {
             hl[j] = lz_hash_long<C::LMLS>(lo, hi);
-            fl[j] = TL[LZ_IDX(hl[j])];
+            fl[j] = TL[LZ_IDX(hl[j])] ^ KX;
         }
     }
     __syncthreads();
+    // the largest key is the tile's earliest position, whatever order the atomics land in
 #pragma unroll
-    for (int j = PPT - 1; j >= 0; j--)                                 // the thread's lowest position lands last
+    for (int j = 0; j < PPT; j++)
         if ((C::INS == 1 || (j & 1) == 0) && (!GUARD || p0 + j < npos)) {
-            TS[LZ_IDX(hs[j])] = LZ_ENT(hs[j], j);
-            if constexpr (C::LONG) TL[LZ_IDX(hl[j])] = LZ_ENT(hl[j], j);
+            atomicMax(&TS[LZ_IDX(hs[j])], LZ_ENT(hs[j], j) ^ KX);
+            if constexpr (C::LONG) atomicMax(&TL[LZ_IDX(hl[j])], LZ_ENT(hl[j], j) ^ KX);
         }
-    __syncthreads();
-    {
-        // all slots are read before the first fix: the loads overlap (an atomic between two loads would order them), and a
-        // stale value can only cause a redundant atomicMin
-        uint32_t cs[PPT], cl[C::LONG ? PPT : 1];
-#pragma unroll
-        for (int j = 0; j < PPT; j++)
-            if (C::INS == 1 || (j & 1) == 0) {
-                cs[j] = TS[LZ_IDX(hs[j])];
-                if constexpr (C::LONG) cl[j] = TL[LZ_IDX(hl[j])];
-            }
-#pragma unroll
-        for (int j = 0; j < PPT; j++)
-            if ((C::INS == 1 || (j & 1) == 0) && (!GUARD || p0 + j < npos)) {
-                if (cs[j] > LZ_ENT(hs[j], j)) atomicMin(&TS[LZ_IDX(hs[j])], LZ_ENT(hs[j], j));   // lost a store race: exact minimum of the tile
-                if constexpr (C::LONG) { if (cl[j] > LZ_ENT(hl[j], j)) atomicMin(&TL[LZ_IDX(hl[j])], LZ_ENT(hl[j], j)); }
-            }
-    }
     __syncthreads();
     uint32_t bitsA = 0, bitsL = 0, dist[PPT];
 #pragma unroll
@@ -248,14 +241,14 @@ B2C_DEV void lz_dense_tile(uint32_t *TS, uint32_t *TL, uint32_t *bm, uint32_t *b
         if (!GUARD || p0 + j < npos) {
             if constexpr (C::LONG) {
                 const uint32_t e = LZ_ENT(hl[j], j);
-                const uint32_t tn = e - TL[LZ_IDX(hl[j])], tf = e - fl[j];
+                const uint32_t tn = e - (TL[LZ_IDX(hl[j])] ^ KX), tf = e - fl[j];
                 const bool nearOk = (tn & BAD) == 0 && tn != 0;           // near: the tile's earliest equal-hash position, if before this one
                 okL = nearOk || (tf & BAD) == 0;
                 if (okL) d = (nearOk ? tn : tf) >> LZ_TAGBITS;
             }
             if (!okL) {
                 const uint32_t e = LZ_ENT(hs[j], j);
-                const uint32_t tn = e - TS[LZ_IDX(hs[j])], tf = e - fs[j];
+                const uint32_t tn = e - (TS[LZ_IDX(hs[j])] ^ KX), tf = e - fs[j];
                 const bool nearOk = (tn & BAD) == 0 && tn != 0;
                 ok = nearOk || (tf & BAD) == 0;
                 if (ok) d = (nearOk ? tn : tf) >> LZ_TAGBITS;
@@ -361,7 +354,7 @@ B2C_DEV void lz_parse_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chun
     }
     B2C_PHASE(0);
     // ---------------------------------------------------------------- P0: empty tables
-    for (uint32_t i = tid; i < L::NTAB * TSIZE; i += NT) TS[i] = LZ_EMPTY;
+    for (uint32_t i = tid; i < L::NTAB * TSIZE; i += NT) TS[i] = LZ_EMPTY<NT * C::PPT>;
     if (tid < 16) {
         uint32_t sel = 0, k = 0;
         for (uint32_t bb = 0; bb < 4; bb++)
