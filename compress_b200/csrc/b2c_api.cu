@@ -28,68 +28,85 @@
 
 using namespace b2c;
 
+// Memory the context owns: device or pinned host memory, grown by reserve() and freed with the context.  Every member
+// states where it lives and how it grows where it is declared.  cap is in bytes.
+enum BufKind { kDevice, kPinned };
+enum BufGrowth { kExact, kHeadroom };   // kHeadroom: 25 % more than asked for, so that slowly rising sizes do not regrow each call
+template <class T = uint8_t> struct Buf {
+    const BufKind kind;
+    const BufGrowth growth;
+    T *p = nullptr;
+    size_t cap = 0;
+    Buf(BufKind k, BufGrowth g) : kind(k), growth(g) {}
+    Buf(const Buf &) = delete;
+    Buf &operator=(const Buf &) = delete;
+    ~Buf() { if (p) { if (kind == kPinned) cudaFreeHost(p); else cudaFree(p); } }
+    template <class U> U *at(size_t off) const { return reinterpret_cast<U *>(reinterpret_cast<uint8_t *>(p) + off); }
+};
+// An event or stream the context owns, destroyed with it.
+template <class H, cudaError_t (*destroy)(H)> struct Owned {
+    H h = nullptr;
+    Owned() = default;
+    Owned(const Owned &) = delete;
+    Owned &operator=(const Owned &) = delete;
+    ~Owned() { if (h) destroy(h); }
+    operator H() const { return h; }
+};
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+
+// One slot of the encode pipeline.  b2c_zstd_encode_packed alternates batches between the two slots (H2D / kernels / D2H
+// overlap); every other encode call uses slot 0.  The host-buffer buffers hold max_chunks chunks of 64 KiB.
+struct EncSlot {
+    Buf<> d_in{kDevice, kExact}, d_out{kDevice, kExact};      // input chunks | output slots of kSlot bytes
+    Buf<> d_packed{kDevice, kExact};                          // the batch's frames back to back
+    Buf<int64_t> d_sizes{kDevice, kExact}, h_sizes{kPinned, kExact};   // h_sizes: sizes | packed offsets
+    Buf<uint64_t> d_offsets{kDevice, kExact};
+    Buf<uint32_t> d_src_sizes{kDevice, kExact}, h_src_sizes{kPinned, kExact};
+    Buf<> h_in{kPinned, kExact}, h_out{kPinned, kExact};      // pinned staging (slot 1's: allocated for the first pageable caller)
+    Buf<ChunkWork> work{kDevice, kExact};                     // per-chunk work records, grown on demand
+    Buf<> pool{kDevice, kExact};                              // per-chunk work pool slabs (literals, sequences, codes, state bits)
+    size_t scratch_off = 0;                                   // this slot's set of the per-CTA parse scratch
+    Event ev, ev_in, ev_out;                                  // compute / H2D / D2H of the slot's batch finished
+};
+
 struct b2c_ctx {
     int device = 0;
     int sm_count = 0;
     size_t max_chunks = 0;
-    uint8_t *d_scratch = nullptr;       // per-CTA parse scratch (two sets: one per pipeline slot)
-    size_t scratch_slot = 0;            // bytes of one set
-    ChunkWork *d_work[2] = {nullptr, nullptr};   // per-chunk work records, grown on demand
-    uint8_t *d_pool[2] = {nullptr, nullptr};     // per-chunk work pool slabs (literals, sequences, codes, state bits)
-    size_t work_cap[2] = {0, 0};        // chunks the records hold
-    size_t pool_cap[2] = {0, 0};        // bytes
-    cudaEvent_t ev_busy = nullptr;      // last launch that used the context's scratch / work buffers
+    Stream stream;                      // every host-buffer call; the kernels of b2c_zstd_encode_packed
+    Stream stream2, stream3;            // b2c_zstd_encode_packed: H2D / D2H
+    Stream dec_aux;                     // staged decode: the literal kernel runs beside the sequence walk
+    Event ev_busy;                      // last launch that used the context's scratch / work buffers
     cudaStream_t busy_stream = nullptr; bool busy_valid = false;
-    // host-buffer path staging (slot 0 of the pipeline doubles as the pointer-table path's buffers)
-    uint8_t *h_in = nullptr;            // pinned, max_chunks * 64 KiB
-    uint8_t *h_out = nullptr;           // pinned, max_chunks * slot
-    int64_t *h_sizes = nullptr;         // pinned
-    uint8_t *d_in = nullptr;
-    uint8_t *d_out = nullptr;           // slots
-    uint8_t *d_packed = nullptr;        // packed output
-    int64_t *d_sizes = nullptr;
-    uint64_t *d_offsets = nullptr;
-    uint32_t *d_src_sizes = nullptr;
-    uint32_t *h_src_sizes = nullptr;
-    cudaStream_t stream = nullptr;
-    // second pipeline slot for b2c_zstd_encode_packed (H2D / encode / D2H overlap)
-    uint8_t *d_in2 = nullptr, *d_out2 = nullptr, *d_packed2 = nullptr;
-    int64_t *d_sizes2 = nullptr, *h_sizes2 = nullptr;
-    uint64_t *d_offsets2 = nullptr;
-    uint32_t *d_src_sizes2 = nullptr, *h_src_sizes2 = nullptr;
-    cudaStream_t stream2 = nullptr;
-    cudaStream_t stream3 = nullptr;
-    cudaStream_t dec_aux = nullptr;                        // staged decode: the literal kernel runs beside the sequence walk
-    uint8_t *d_fr = nullptr; size_t fr_cap = 0;            // frame mode: block / frame tables, block slots (grown on demand)
-    uint8_t *d_fr_io = nullptr; size_t fr_io_cap = 0;      // frame mode, host-buffer call: staged input | packed output | results
-    uint8_t *d_s2d = nullptr; size_t s2d_cap = 0;          // staged S2 block decode: block heads + element records
-    uint8_t *d_s2s = nullptr; size_t s2s_cap = 0;          // S2 stream calls: block slots, sizes, checksums, scan, tables (grown on demand)
-    uint8_t *d_s2s_io = nullptr; size_t s2s_io_cap = 0;    //   host-buffer calls: staged input | output
-    uint32_t *d_counters = nullptr; uint32_t counter_seq = 0;   // chunk counters of the persistent parse kernels (one per launch, rotating)
+    Event dec_fork, dec_join;
+    Buf<> d_scratch{kDevice, kExact};   // per-CTA parse scratch (two sets: one per pipeline slot)
+    EncSlot slot[2];
+    Buf<> d_fr{kDevice, kExact};        // frame mode: block / frame tables, block slots (grown on demand)
+    Buf<> d_fr_io{kDevice, kExact};     // frame mode, host-buffer call: staged input | packed output | results
+    Buf<> d_s2d{kDevice, kHeadroom};    // staged S2 block decode: block heads + element records
+    Buf<> d_s2s{kDevice, kExact};       // S2 stream calls: block slots, sizes, checksums, scan, tables (grown on demand)
+    Buf<> d_s2s_io{kDevice, kExact};    //   host-buffer calls: staged input | output
+    Buf<uint32_t> d_counters{kDevice, kExact}; uint32_t counter_seq = 0;   // chunk counters of the persistent parse kernels (one per launch, rotating)
     int enc_fused_xxh = 1;                                 // B2C_ENC_XXH=kernel: XXH64 as its own kernel (A/B measurements)
-    cudaEvent_t dec_fork = nullptr, dec_join = nullptr;
-    uint8_t *h_in2 = nullptr, *h_out2 = nullptr;   // second pinned staging pair: pageable callers of b2c_zstd_encode_packed (lazy)
-    cudaEvent_t ev[2] = {nullptr, nullptr};       // compute of the batch in slot s finished
-    cudaEvent_t ev_in[2] = {nullptr, nullptr};    // H2D of slot s finished
-    cudaEvent_t ev_out[2] = {nullptr, nullptr};   // D2H of slot s finished
     // decoder: per-warp literal scratch, host-path staging (grown on demand)
-    uint8_t *d_dec_lit = nullptr; size_t dec_lit_cap = 0;
-    uint8_t *d_fd = nullptr; size_t fd_cap = 0;            // staged decoder: records | FSE tables | Huffman tables
-    uint32_t *d_fd_const = nullptr;                          //   code maps + predefined tables
-    uint8_t *d_fd_seq = nullptr; size_t fd_seq_cap = 0;    //   sequence records
-    uint8_t *d_fd_lit = nullptr; size_t fd_lit_cap = 0;    //   decoded literals
+    Buf<> d_dec_lit{kDevice, kHeadroom};
+    Buf<> d_fd{kDevice, kHeadroom};                        // staged decoder: records | FSE tables | Huffman tables
+    Buf<uint32_t> d_fd_const{kDevice, kExact};             //   code maps + predefined tables
+    Buf<> d_fd_seq{kDevice, kHeadroom};                    //   sequence records
+    Buf<> d_fd_lit{kDevice, kHeadroom};                    //   decoded literals
     int dec_staged = 1;                                    // B2C_DEC=onewarp: one-warp decoder only (A/B measurements)
-    bool fd_last = false, s2d_last = false;                // the most recent zstd / S2 decode launch ran the staged kernels
-    float dec_ms[6] = {0, 0, 0, 0, 0, 0}; cudaEvent_t dec_ev[7] = {}; int dec_prof = 0;
-    uint8_t *d_dec_in = nullptr, *d_dec_out = nullptr; size_t dec_in_cap = 0, dec_out_cap = 0;
-    uint8_t *d_dec_meta = nullptr; size_t dec_meta_cap = 0;
-    uint8_t *h_stg_in = nullptr, *h_stg_out = nullptr; size_t h_stg_in_cap = 0, h_stg_out_cap = 0;   // pinned staging of the pointer-table calls
+    bool fd_last = false, s2d_last = false;                // d_fd / d_s2d hold the records of the most recent zstd / S2 decode launch
+    float dec_ms[6] = {0, 0, 0, 0, 0, 0}; Event dec_ev[7]; int dec_prof = 0;
+    Buf<> d_dec_in{kDevice, kHeadroom}, d_dec_out{kDevice, kHeadroom}, d_dec_meta{kDevice, kHeadroom};
+    Buf<> h_stg_in{kPinned, kHeadroom}, h_stg_out{kPinned, kHeadroom};   // pinned staging of the pointer-table calls
     // optional per-kernel timing of the encode pipeline (b2c_profile_*): 6 events per encode call
     bool prof = false;
     std::vector<cudaEvent_t> pev;
     size_t pev_used = 0;
     uint64_t launches = 0;
     char err[256] = {0};
+    ~b2c_ctx() { for (cudaEvent_t e : pev) cudaEventDestroy(e); }
 };
 
 #define CK(call)                                                                                       \
@@ -100,6 +117,26 @@ struct b2c_ctx {
             return B2C_ERR_CUDA;                                                                       \
         }                                                                                              \
     } while (0)
+
+// Grows b to at least `need` bytes; its contents are not kept.  A device buffer is replaced only after the device has
+// synchronised: kernels of earlier calls on other streams may still use the old one.
+template <class T> static int reserve(b2c_ctx *ctx, Buf<T> &b, size_t need) {
+    if (b.cap >= need) return B2C_OK;
+    const bool dev = b.kind == kDevice;
+    if (dev) CK(cudaDeviceSynchronize());
+    if (b.p) CK(dev ? cudaFree(b.p) : cudaFreeHost(b.p));
+    b.p = nullptr; b.cap = 0;
+    if (b.growth == kHeadroom) need += need / 4;
+    CK(dev ? cudaMalloc(&b.p, need) : cudaMallocHost(&b.p, need));
+    b.cap = need;
+    return B2C_OK;
+}
+
+// Pieces of one buffer, each starting 256-byte aligned: take() returns a piece's offset, end is the bytes they span.
+struct Layout {
+    size_t end = 0;
+    size_t take(size_t bytes) { const size_t r = end; end += (bytes + 255) & ~(size_t)255; return r; }
+};
 
 // Host-side gather / scatter of many separately addressed pieces (the pointer-table calls): index ranges are spread over a few
 // host threads when there is enough to move -- one thread copies about 10 GB/s, which otherwise bounds these calls far
@@ -196,6 +233,7 @@ b2c_ctx *b2c_ctx_create(int device, size_t max_chunks) {
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return nullptr; }
     ctx->sm_count = prop.multiProcessorCount;
     bool ok = true;
+    size_t scratch_slot = 0;            // bytes of one slot's scratch set
     {
         size_t a = 0;
         size_t b = (size_t)ctx->sm_count * LzCfg<1>::MIN_CTAS * LzLayout<1>::SCRATCH_BYTES;
@@ -206,54 +244,46 @@ b2c_ctx *b2c_ctx_create(int device, size_t max_chunks) {
         if (d4 > a) a = d4;
         size_t d5 = (size_t)ctx->sm_count * LzCfg<5>::MIN_CTAS * LzLayout<5>::SCRATCH_BYTES;
         if (d5 > a) a = d5;
-        ctx->scratch_slot = ((a > b ? (a > c ? a : c) : (b > c ? b : c)) + 255) & ~(size_t)255;
+        scratch_slot = ((a > b ? (a > c ? a : c) : (b > c ? b : c)) + 255) & ~(size_t)255;
     }
-    ok = ok && cudaMalloc(&ctx->d_scratch, 2 * ctx->scratch_slot) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&ctx->ev_busy, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_parse1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)LzLayout<1>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_parse2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)LzLayout<2>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_parse3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)LzLayout<5>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_s2_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LzLayout<3>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_snappy_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LzLayout<3>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_s2_better_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LzLayout<4>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_lz_snappy_better_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LzLayout<4>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)HIST_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_pack128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)PackCfg<131072>::SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_chains_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)CHAIN_SMEM_BYTES) == cudaSuccess;
+    ok = ok && reserve(ctx, ctx->d_scratch, 2 * scratch_slot) == B2C_OK;
+    ok = ok && cudaEventCreateWithFlags(&ctx->ev_busy.h, cudaEventDisableTiming) == cudaSuccess;
+    const struct { const void *fn; int bytes; } smem[] = {
+        {(const void *)b2c_lz_parse1_kernel, (int)LzLayout<1>::SMEM_BYTES},
+        {(const void *)b2c_lz_parse2_kernel, (int)LzLayout<2>::SMEM_BYTES},
+        {(const void *)b2c_lz_parse3_kernel, (int)LzLayout<5>::SMEM_BYTES},
+        {(const void *)b2c_lz_s2_fast_kernel, (int)LzLayout<3>::SMEM_BYTES},
+        {(const void *)b2c_lz_snappy_fast_kernel, (int)LzLayout<3>::SMEM_BYTES},
+        {(const void *)b2c_lz_s2_better_kernel, (int)LzLayout<4>::SMEM_BYTES},
+        {(const void *)b2c_lz_snappy_better_kernel, (int)LzLayout<4>::SMEM_BYTES},
+        {(const void *)b2c_zstd_hist_kernel, (int)HIST_SMEM_BYTES},
+        {(const void *)b2c_zstd_pack128_kernel, (int)PackCfg<131072>::SMEM_BYTES},
+        {(const void *)b2c_zstd_pack_kernel, (int)PACK_SMEM_BYTES},
+        {(const void *)b2c_zstd_chains_kernel, (int)CHAIN_SMEM_BYTES},
+        {(const void *)b2c_huf_compress_kernel, (int)HUF0_SMEM_BYTES},
+        {(const void *)b2c_huf_decompress_kernel, (int)DEC_SMEM_BYTES},
+        {(const void *)b2c_huf_dec_prep_kernel, (int)DEC_SMEM_BYTES},
+        {(const void *)b2c_huf_read_table_kernel, (int)DEC_SMEM_BYTES},
+        {(const void *)b2c_zstd_decode_kernel, (int)DEC_SMEM_BYTES},
+        {(const void *)b2c_zstd_dec_lit_kernel, (int)(FD_LIT_WARPS * FD_LIT_WARP_BYTES)},
+        {(const void *)b2c_zstd_dec_init_kernel, (int)DEC_WARP_BYTES},
+    };
+    for (const auto &k : smem)
+        ok = ok && cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.bytes) == cudaSuccess;
     // at most two chains CTAs per SM, the rest of the SM's memory stays L1: a 16384-chunk pass (512 CTAs) took
     // 1.21 ms per GiB with four CTAs sharing an SM and 0.99 ms with two (H100 SXM at 700 W, level 1)
     ok = ok && cudaFuncSetAttribute(b2c_zstd_chains_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 50) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_huf_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)HUF0_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_huf_decompress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)DEC_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_huf_dec_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)DEC_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_huf_read_table_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)DEC_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)DEC_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_dec_lit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)(FD_LIT_WARPS * FD_LIT_WARP_BYTES)) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_dec_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)DEC_WARP_BYTES) == cudaSuccess;
-    ok = ok && cudaMalloc(&ctx->d_fd_const, FD_CONST_ENTRIES * sizeof(uint32_t)) == cudaSuccess;
+    ok = ok && cudaStreamCreateWithFlags(&ctx->stream.h, cudaStreamNonBlocking) == cudaSuccess;
+    ok = ok && reserve(ctx, ctx->d_fd_const, FD_CONST_ENTRIES * sizeof(uint32_t)) == B2C_OK;
     if (ok) {
-        b2c_zstd_dec_init_kernel<<<1, 32, DEC_WARP_BYTES>>>(ctx->d_fd_const);
+        b2c_zstd_dec_init_kernel<<<1, 32, DEC_WARP_BYTES>>>(ctx->d_fd_const.p);
         ok = cudaDeviceSynchronize() == cudaSuccess;
     }
-    for (int i = 0; i < 7; i++) ok = ok && cudaEventCreate(&ctx->dec_ev[i]) == cudaSuccess;
-    ok = ok && cudaStreamCreateWithFlags(&ctx->dec_aux, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&ctx->dec_fork, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&ctx->dec_join, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaMalloc(&ctx->d_counters, 256 * sizeof(uint32_t)) == cudaSuccess;
+    for (Event &e : ctx->dec_ev) ok = ok && cudaEventCreate(&e.h) == cudaSuccess;
+    ok = ok && cudaStreamCreateWithFlags(&ctx->dec_aux.h, cudaStreamNonBlocking) == cudaSuccess;
+    ok = ok && cudaEventCreateWithFlags(&ctx->dec_fork.h, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && cudaEventCreateWithFlags(&ctx->dec_join.h, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && reserve(ctx, ctx->d_counters, 256 * sizeof(uint32_t)) == B2C_OK;
     {
         const char *es = getenv("B2C_ENC_XXH");
         ctx->enc_fused_xxh = (es && strcmp(es, "kernel") == 0) ? 0 : 1;
@@ -262,34 +292,28 @@ b2c_ctx *b2c_ctx_create(int device, size_t max_chunks) {
         const char *de = getenv("B2C_DEC");
         ctx->dec_staged = (de && strcmp(de, "onewarp") == 0) ? 0 : 1;
     }
-    ok = ok && cudaFuncSetAttribute(b2c_zstd_pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)PACK_SMEM_BYTES) == cudaSuccess;
     if (ok && max_chunks) {
-        ok = ok && cudaMallocHost(&ctx->h_in, max_chunks * (size_t)ENC_MAX_CHUNK) == cudaSuccess;
-        ok = ok && cudaMallocHost(&ctx->h_out, max_chunks * (size_t)kSlot) == cudaSuccess;
-        ok = ok && cudaMallocHost(&ctx->h_sizes, (max_chunks + 1) * sizeof(int64_t) * 2) == cudaSuccess;
-        ok = ok && cudaMallocHost(&ctx->h_src_sizes, max_chunks * sizeof(uint32_t)) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_in, max_chunks * (size_t)ENC_MAX_CHUNK) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_out, max_chunks * (size_t)kSlot) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_packed, max_chunks * (size_t)kSlot) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_sizes, max_chunks * sizeof(int64_t)) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_offsets, (max_chunks + 1) * sizeof(uint64_t)) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_src_sizes, max_chunks * sizeof(uint32_t)) == cudaSuccess;
-        ok = ok && cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking) == cudaSuccess;
-        ok = ok && cudaStreamCreateWithFlags(&ctx->stream3, cudaStreamNonBlocking) == cudaSuccess;
-        for (int k = 0; k < 2; k++) {
-            ok = ok && cudaEventCreateWithFlags(&ctx->ev[k], cudaEventDisableTiming) == cudaSuccess;
-            ok = ok && cudaEventCreateWithFlags(&ctx->ev_in[k], cudaEventDisableTiming) == cudaSuccess;
-            ok = ok && cudaEventCreateWithFlags(&ctx->ev_out[k], cudaEventDisableTiming) == cudaSuccess;
+        ok = ok && cudaStreamCreateWithFlags(&ctx->stream2.h, cudaStreamNonBlocking) == cudaSuccess;
+        ok = ok && cudaStreamCreateWithFlags(&ctx->stream3.h, cudaStreamNonBlocking) == cudaSuccess;
+    }
+    for (int k = 0; k < 2; k++) {
+        EncSlot &S = ctx->slot[k];
+        S.scratch_off = k * scratch_slot;
+        if (!ok || !max_chunks) continue;
+        ok = ok && reserve(ctx, S.d_in, max_chunks * (size_t)ENC_MAX_CHUNK) == B2C_OK;
+        ok = ok && reserve(ctx, S.d_out, max_chunks * (size_t)kSlot) == B2C_OK;
+        ok = ok && reserve(ctx, S.d_packed, max_chunks * (size_t)kSlot) == B2C_OK;
+        ok = ok && reserve(ctx, S.d_sizes, max_chunks * sizeof(int64_t)) == B2C_OK;
+        ok = ok && reserve(ctx, S.h_sizes, (max_chunks + 1) * sizeof(int64_t) * 2) == B2C_OK;
+        ok = ok && reserve(ctx, S.d_offsets, (max_chunks + 1) * sizeof(uint64_t)) == B2C_OK;
+        ok = ok && reserve(ctx, S.d_src_sizes, max_chunks * sizeof(uint32_t)) == B2C_OK;
+        ok = ok && reserve(ctx, S.h_src_sizes, max_chunks * sizeof(uint32_t)) == B2C_OK;
+        if (k == 0) {       // slot 1's staging is allocated by the first pageable caller of b2c_zstd_encode_packed
+            ok = ok && reserve(ctx, S.h_in, max_chunks * (size_t)ENC_MAX_CHUNK) == B2C_OK;
+            ok = ok && reserve(ctx, S.h_out, max_chunks * (size_t)kSlot) == B2C_OK;
         }
-        ok = ok && cudaMallocHost(&ctx->h_sizes2, (max_chunks + 1) * sizeof(int64_t) * 2) == cudaSuccess;
-        ok = ok && cudaMallocHost(&ctx->h_src_sizes2, max_chunks * sizeof(uint32_t)) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_in2, max_chunks * (size_t)ENC_MAX_CHUNK) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_out2, max_chunks * (size_t)kSlot) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_packed2, max_chunks * (size_t)kSlot) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_sizes2, max_chunks * sizeof(int64_t)) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_offsets2, (max_chunks + 1) * sizeof(uint64_t)) == cudaSuccess;
-        ok = ok && cudaMalloc(&ctx->d_src_sizes2, max_chunks * sizeof(uint32_t)) == cudaSuccess;
+        for (Event *e : {&S.ev, &S.ev_in, &S.ev_out})
+            ok = ok && cudaEventCreateWithFlags(&e->h, cudaEventDisableTiming) == cudaSuccess;
     }
     if (!ok) { b2c_ctx_destroy(ctx); return nullptr; }
     return ctx;
@@ -298,29 +322,7 @@ b2c_ctx *b2c_ctx_create(int device, size_t max_chunks) {
 void b2c_ctx_destroy(b2c_ctx *ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    cudaFreeHost(ctx->h_stg_in); cudaFreeHost(ctx->h_stg_out);
-    cudaFree(ctx->d_fd); cudaFree(ctx->d_fd_const); cudaFree(ctx->d_fd_seq); cudaFree(ctx->d_fd_lit);
-    cudaFree(ctx->d_dec_lit); cudaFree(ctx->d_dec_in); cudaFree(ctx->d_dec_out); cudaFree(ctx->d_dec_meta);
-    cudaFree(ctx->d_fr); cudaFree(ctx->d_fr_io); cudaFree(ctx->d_counters); cudaFree(ctx->d_s2s); cudaFree(ctx->d_s2s_io); cudaFree(ctx->d_s2d);
-    cudaFree(ctx->d_scratch); cudaFree(ctx->d_work[0]); cudaFree(ctx->d_work[1]); cudaFree(ctx->d_pool[0]); cudaFree(ctx->d_pool[1]);
-    if (ctx->ev_busy) cudaEventDestroy(ctx->ev_busy); cudaFree(ctx->d_in); cudaFree(ctx->d_out); cudaFree(ctx->d_packed);
-    cudaFree(ctx->d_sizes); cudaFree(ctx->d_offsets); cudaFree(ctx->d_src_sizes);
-    cudaFreeHost(ctx->h_in); cudaFreeHost(ctx->h_out); cudaFreeHost(ctx->h_in2); cudaFreeHost(ctx->h_out2); cudaFreeHost(ctx->h_sizes); cudaFreeHost(ctx->h_src_sizes);
-    cudaFree(ctx->d_in2); cudaFree(ctx->d_out2); cudaFree(ctx->d_packed2); cudaFree(ctx->d_sizes2);
-    cudaFree(ctx->d_offsets2); cudaFree(ctx->d_src_sizes2); cudaFreeHost(ctx->h_sizes2); cudaFreeHost(ctx->h_src_sizes2);
-    for (cudaEvent_t e : ctx->pev) cudaEventDestroy(e);
-    for (int k = 0; k < 2; k++) {
-        if (ctx->ev[k]) cudaEventDestroy(ctx->ev[k]);
-        if (ctx->ev_in[k]) cudaEventDestroy(ctx->ev_in[k]);
-        if (ctx->ev_out[k]) cudaEventDestroy(ctx->ev_out[k]);
-    }
-    if (ctx->dec_aux) cudaStreamDestroy(ctx->dec_aux);
-    if (ctx->dec_fork) cudaEventDestroy(ctx->dec_fork);
-    if (ctx->dec_join) cudaEventDestroy(ctx->dec_join);
-    if (ctx->stream3) cudaStreamDestroy(ctx->stream3);
-    if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;             // the members free the buffers and destroy the events and streams they hold
 }
 
 const char *b2c_strerror(int code) {
@@ -393,29 +395,27 @@ static int staged_flags(b2c_ctx *ctx, const uint8_t *recs, bool last, size_t rec
 // through the one-warp decoder.  Synchronises the device.  Test / diagnostics hook.
 int b2c_decode_staged_flags(b2c_ctx *ctx, uint32_t nchunks, uint8_t *flags) {
     if (!ctx || (!flags && nchunks)) return B2C_ERR_ARG;
-    return staged_flags(ctx, ctx->d_fd, ctx->fd_last, sizeof(FdChunk), ctx->fd_cap, nchunks, flags);
+    return staged_flags(ctx, ctx->d_fd.p, ctx->fd_last, sizeof(FdChunk), ctx->d_fd.cap, nchunks, flags);
 }
 // The same for the most recent S2 block decode launch: blocks finished by the staged kernels (tag walk + execution).
 int b2c_s2_decode_staged_flags(b2c_ctx *ctx, uint32_t nchunks, uint8_t *flags) {
     if (!ctx || (!flags && nchunks)) return B2C_ERR_ARG;
-    return staged_flags(ctx, ctx->d_s2d, ctx->s2d_last, sizeof(S2Head), ctx->s2d_cap, nchunks, flags);
+    return staged_flags(ctx, ctx->d_s2d.p, ctx->s2d_last, sizeof(S2Head), ctx->d_s2d.cap, nchunks, flags);
 }
-// How many of the first nchunks inputs of the most recent decode launch the staged kernels completed.
-int b2c_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
+// How many of the first nchunks inputs of the most recent (S2) decode launch the staged kernels completed.
+static int staged_count(int (*flags_of)(b2c_ctx *, uint32_t, uint8_t *), b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
     if (!ctx || !staged) return B2C_ERR_ARG;
     std::vector<uint8_t> f(nchunks);
-    const int rc = b2c_decode_staged_flags(ctx, nchunks, f.data());
+    const int rc = flags_of(ctx, nchunks, f.data());
     *staged = 0;
     for (uint8_t v : f) *staged += v;
     return rc;
+}
+int b2c_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
+    return staged_count(b2c_decode_staged_flags, ctx, nchunks, staged);
 }
 int b2c_s2_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged) {
-    if (!ctx || !staged) return B2C_ERR_ARG;
-    std::vector<uint8_t> f(nchunks);
-    const int rc = b2c_s2_decode_staged_flags(ctx, nchunks, f.data());
-    *staged = 0;
-    for (uint8_t v : f) *staged += v;
-    return rc;
+    return staged_count(b2c_s2_decode_staged_flags, ctx, nchunks, staged);
 }
 int b2c_decode_profile_read(b2c_ctx *ctx, double *ms) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
@@ -438,7 +438,7 @@ size_t b2c_zstd_bound(size_t size, int level) {
 
 // a zeroed chunk counter for one launch of a persistent parse kernel (rotating: launches in flight never share one)
 static int next_counter(b2c_ctx *ctx, cudaStream_t st, uint32_t **out) {
-    uint32_t *c = ctx->d_counters + (ctx->counter_seq++ & 255u);
+    uint32_t *c = ctx->d_counters.p + (ctx->counter_seq++ & 255u);
     CK(cudaMemsetAsync(c, 0, sizeof(uint32_t), st));
     *out = c;
     return B2C_OK;
@@ -479,22 +479,9 @@ static int launch_encode(b2c_ctx *ctx, int level, int flags, const void *d_src, 
     // 64 KiB chunk (5.7 GB at 16384), 821 KB per 128 KiB block (6.7 GB at 8192); it grows only for calls that large.
     const uint32_t subMax = blockmax > 65536 ? 8192u : 16384u;
     const uint32_t sub = nchunks < subMax ? nchunks : subMax;
-    if (ctx->work_cap[slot] < sub || ctx->pool_cap[slot] < (size_t)sub * pstride) {
-        // grow the per-chunk work records / pool (kernels of earlier calls on other streams may still use the old ones)
-        CK(cudaDeviceSynchronize());
-        if (ctx->work_cap[slot] < sub) {
-            if (ctx->d_work[slot]) CK(cudaFree(ctx->d_work[slot]));
-            ctx->d_work[slot] = nullptr; ctx->work_cap[slot] = 0;
-            CK(cudaMalloc(&ctx->d_work[slot], (size_t)sub * sizeof(ChunkWork)));
-            ctx->work_cap[slot] = sub;
-        }
-        if (ctx->pool_cap[slot] < (size_t)sub * pstride) {
-            if (ctx->d_pool[slot]) CK(cudaFree(ctx->d_pool[slot]));
-            ctx->d_pool[slot] = nullptr; ctx->pool_cap[slot] = 0;
-            CK(cudaMalloc(&ctx->d_pool[slot], (size_t)sub * pstride));
-            ctx->pool_cap[slot] = (size_t)sub * pstride;
-        }
-    }
+    EncSlot &S = ctx->slot[slot];
+    { int r = reserve(ctx, S.work, (size_t)sub * sizeof(ChunkWork)); if (r) return r; }
+    { int r = reserve(ctx, S.pool, (size_t)sub * pstride); if (r) return r; }
     { int r = ctx_order_begin(ctx, st); if (r) return r; }
     const unsigned sms = (unsigned)ctx->sm_count;
     for (uint32_t c0 = 0; c0 < nchunks; c0 += sub) {
@@ -506,9 +493,9 @@ static int launch_encode(b2c_ctx *ctx, int level, int flags, const void *d_src, 
         P.src_sizes = d_sizes ? d_sizes + c0 : nullptr; P.src_size_all = size_all;
         P.dst_base = (uint8_t *)d_dst + (size_t)c0 * dst_stride; P.dst_stride = dst_stride; P.dst_cap = (uint32_t)dst_stride;
         P.out_sizes = d_out_sizes + c0; P.nchunks = m; P.flags = (uint32_t)flags;
-        P.scratch = ctx->d_scratch + (size_t)slot * ctx->scratch_slot;
-        P.work = ctx->d_work[slot];
-        P.pool = ctx->d_pool[slot]; P.pool_stride = pstride; P.maxseq = wk_maxseq(blockmax); P.blockmax = blockmax;
+        P.scratch = ctx->d_scratch.p + S.scratch_off;
+        P.work = S.work.p;
+        P.pool = S.pool.p; P.pool_stride = pstride; P.maxseq = wk_maxseq(blockmax); P.blockmax = blockmax;
         P.big = blockmax > 65536 ? 1u : 0u; P.level = (uint32_t)level;
         if (dbg_hdr) {
             P.dbg_hdr = dbg_hdr + (size_t)c0 * 4; P.dbg_seqs = dbg_seqs + (size_t)c0 * dbg_cap * 3;
@@ -653,27 +640,20 @@ int b2c_zstd_encode_frames_device(b2c_ctx *ctx, int level, int flags, const void
     const uint32_t sub = nblocks < subMax ? nblocks : subMax, nsub = (nblocks + sub - 1) / sub;
     const size_t slotB = (size_t)g.block + 512;
     // ---- device memory of the call: descriptors | frame table | per-block sizes, positions | scan offsets | bases | xxh | slots
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-    const size_t oDesc = take(sizeof(EncBlockDesc) * nblocks), oFr = take(sizeof(FrameDesc) * nframes),
-                 oSizes = take(sizeof(int64_t) * nblocks), oPos = take(sizeof(uint64_t) * nblocks),
-                 oScan = take(sizeof(uint64_t) * ((size_t)sub + 1)), oBase = take(sizeof(uint64_t) * ((size_t)nsub + 1)),
-                 oXxh = take(sizeof(uint64_t) * nframes), oSlots = take(slotB * sub);
-    if (ctx->fr_cap < o) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->d_fr) CK(cudaFree(ctx->d_fr));
-        ctx->d_fr = nullptr; ctx->fr_cap = 0;
-        CK(cudaMalloc(&ctx->d_fr, o));
-        ctx->fr_cap = o;
-    }
+    Layout L;
+    const size_t oDesc = L.take(sizeof(EncBlockDesc) * nblocks), oFr = L.take(sizeof(FrameDesc) * nframes),
+                 oSizes = L.take(sizeof(int64_t) * nblocks), oPos = L.take(sizeof(uint64_t) * nblocks),
+                 oScan = L.take(sizeof(uint64_t) * ((size_t)sub + 1)), oBase = L.take(sizeof(uint64_t) * ((size_t)nsub + 1)),
+                 oXxh = L.take(sizeof(uint64_t) * nframes), oSlots = L.take(slotB * sub);
+    { int r = reserve(ctx, ctx->d_fr, L.end); if (r) return r; }
     { int r = ctx_order_begin(ctx, st); if (r) return r; }   // (the frame buffers belong to the context like the work pool)
-    uint8_t *B = ctx->d_fr;
-    EncBlockDesc *d_desc = (EncBlockDesc *)(B + oDesc);
-    FrameDesc *d_frames = (FrameDesc *)(B + oFr);
-    int64_t *d_sizes = (int64_t *)(B + oSizes);
-    uint64_t *d_pos = (uint64_t *)(B + oPos), *d_scan = (uint64_t *)(B + oScan), *d_base = (uint64_t *)(B + oBase),
-             *d_xxh = (uint64_t *)(B + oXxh);
-    uint8_t *d_slots = B + oSlots;
+    const Buf<> &B = ctx->d_fr;
+    EncBlockDesc *d_desc = B.at<EncBlockDesc>(oDesc);
+    FrameDesc *d_frames = B.at<FrameDesc>(oFr);
+    int64_t *d_sizes = B.at<int64_t>(oSizes);
+    uint64_t *d_pos = B.at<uint64_t>(oPos), *d_scan = B.at<uint64_t>(oScan), *d_base = B.at<uint64_t>(oBase),
+             *d_xxh = B.at<uint64_t>(oXxh);
+    uint8_t *d_slots = B.at<uint8_t>(oSlots);
     // pageable host vectors: the copies complete before cudaMemcpyAsync returns (staged by the runtime)
     CK(cudaMemcpyAsync(d_desc, blocks.data(), sizeof(EncBlockDesc) * nblocks, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_frames, frames.data(), sizeof(FrameDesc) * nframes, cudaMemcpyHostToDevice, st));
@@ -719,15 +699,11 @@ int b2c_zstd_encode_frames(b2c_ctx *ctx, int level, int flags, const void *const
         tout += b2c_zstd_frame_bound(src_sizes[i], level);
     }
     const size_t inB = tin + 64, outB = tout + 64, metaB = (sizeof(uint64_t) + sizeof(int64_t)) * n;
-    if (ctx->fr_io_cap < inB + outB + metaB + 512) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->d_fr_io) CK(cudaFree(ctx->d_fr_io));
-        ctx->d_fr_io = nullptr; ctx->fr_io_cap = 0;
-        CK(cudaMalloc(&ctx->d_fr_io, inB + outB + metaB + 512));
-        ctx->fr_io_cap = inB + outB + metaB + 512;
-    }
-    uint8_t *d_in = ctx->d_fr_io, *d_out = d_in + ((inB + 255) & ~(size_t)255);
-    uint64_t *d_off = (uint64_t *)(d_out + ((outB + 255) & ~(size_t)255));
+    Layout L;
+    const size_t oIn = L.take(inB), oOut = L.take(outB), oMeta = L.take(metaB);   // meta: frame offsets | frame sizes
+    { int r = reserve(ctx, ctx->d_fr_io, inB + outB + metaB + 512); if (r) return r; }   // (512: the rounding of in and out)
+    uint8_t *d_in = ctx->d_fr_io.at<uint8_t>(oIn), *d_out = ctx->d_fr_io.at<uint8_t>(oOut);
+    uint64_t *d_off = ctx->d_fr_io.at<uint64_t>(oMeta);
     int64_t *d_sz = (int64_t *)(d_off + n);
     for (size_t i = 0; i < n; i++)
         if (src_sizes[i]) CK(cudaMemcpyAsync(d_in + offs[i], srcs[i], src_sizes[i], cudaMemcpyHostToDevice, st));
@@ -757,6 +733,7 @@ int b2c_zstd_encode_chunks(b2c_ctx *ctx, int level, int flags, const void *const
     if (!mcap) return B2C_ERR_ARG;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
+    EncSlot &S = ctx->slot[0];
     for (size_t base = 0; base < n; base += mcap) {
         size_t m = n - base;
         if (m > mcap) m = mcap;
@@ -767,39 +744,39 @@ int b2c_zstd_encode_chunks(b2c_ctx *ctx, int level, int flags, const void *const
             if (i + 1 < m && ((const uint8_t *)srcs[base + i] + src_sizes[base + i] != (const uint8_t *)srcs[base + i + 1] ||
                               src_sizes[base + i] != blk))
                 contiguous = false;
-            ctx->h_src_sizes[i] = (uint32_t)(src_sizes[base + i] > blk ? blk + 1 : src_sizes[base + i]);
+            S.h_src_sizes.p[i] = (uint32_t)(src_sizes[base + i] > blk ? blk + 1 : src_sizes[base + i]);
         }
         size_t in_bytes = 0;
         for (size_t i = 0; i < m; i++) in_bytes += src_sizes[base + i];
         if (contiguous) {
-            CK(cudaMemcpyAsync(ctx->d_in, srcs[base], in_bytes, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(S.d_in.p, srcs[base], in_bytes, cudaMemcpyHostToDevice, st));
         } else {
             {
-                uint8_t *hin = ctx->h_in;
+                uint8_t *hin = S.h_in.p;
                 parallel_pieces(m, in_bytes, [=](size_t i) {
                     const size_t sz = src_sizes[base + i] > blk ? 0 : src_sizes[base + i];
                     memcpy(hin + i * (size_t)blk, srcs[base + i], sz);
                 });
             }
-            CK(cudaMemcpyAsync(ctx->d_in, ctx->h_in, m * (size_t)blk, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(S.d_in.p, S.h_in.p, m * (size_t)blk, cudaMemcpyHostToDevice, st));
         }
-        CK(cudaMemcpyAsync(ctx->d_src_sizes, ctx->h_src_sizes, m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-        int rc = launch_encode(ctx, level, flags, ctx->d_in, blk, ctx->d_src_sizes, 0, ctx->d_out, slotB,
-                               ctx->d_sizes, (uint32_t)m, nullptr, nullptr, nullptr, 0, st);
+        CK(cudaMemcpyAsync(S.d_src_sizes.p, S.h_src_sizes.p, m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        int rc = launch_encode(ctx, level, flags, S.d_in.p, blk, S.d_src_sizes.p, 0, S.d_out.p, slotB,
+                               S.d_sizes.p, (uint32_t)m, nullptr, nullptr, nullptr, 0, st);
         if (rc) return rc;
-        b2c_scan_sizes_kernel<<<1, 1024, 0, st>>>(ctx->d_sizes, ctx->d_offsets, (uint32_t)m);
-        b2c_pack_kernel<<<ctx->sm_count * 4, 256, 0, st>>>(ctx->d_out, slotB, ctx->d_sizes, ctx->d_offsets, ctx->d_packed, (uint32_t)m);
+        b2c_scan_sizes_kernel<<<1, 1024, 0, st>>>(S.d_sizes.p, S.d_offsets.p, (uint32_t)m);
+        b2c_pack_kernel<<<ctx->sm_count * 4, 256, 0, st>>>(S.d_out.p, slotB, S.d_sizes.p, S.d_offsets.p, S.d_packed.p, (uint32_t)m);
         ctx->launches += 2;
-        int64_t *h_sz = ctx->h_sizes;
-        uint64_t *h_off = reinterpret_cast<uint64_t *>(ctx->h_sizes + m);
-        CK(cudaMemcpyAsync(h_sz, ctx->d_sizes, m * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(h_off, ctx->d_offsets, (m + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        int64_t *h_sz = S.h_sizes.p;
+        uint64_t *h_off = reinterpret_cast<uint64_t *>(h_sz + m);
+        CK(cudaMemcpyAsync(h_sz, S.d_sizes.p, m * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(h_off, S.d_offsets.p, (m + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         uint64_t total = h_off[m];
-        CK(cudaMemcpyAsync(ctx->h_out, ctx->d_packed, total, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(S.h_out.p, S.d_packed.p, total, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         {
-            const uint8_t *hout = ctx->h_out;
+            const uint8_t *hout = S.h_out.p;
             parallel_pieces(m, (size_t)total, [=](size_t i) {
                 int64_t sz = h_sz[i];
                 if (sz > 0 && (size_t)sz > dst_caps[base + i]) sz = B2C_ERR_DST_SMALL;
@@ -878,43 +855,38 @@ static int encode_packed_impl(b2c_ctx *ctx, int level, int flags, const void *h_
     // pageable caller memory is staged through the context's pinned buffers (see parallel_memcpy above)
     const bool stage_in = src_bytes > 0 && !host_ptr_is_pinned(h_src);
     const bool stage_out = !host_ptr_is_pinned(h_dst);
-    if ((stage_in && !ctx->h_in2) || (stage_out && !ctx->h_out2)) {
-        if (!ctx->h_in2) CK(cudaMallocHost(&ctx->h_in2, ctx->max_chunks * (size_t)ENC_MAX_CHUNK));
-        if (!ctx->h_out2) CK(cudaMallocHost(&ctx->h_out2, ctx->max_chunks * (size_t)kSlot));
+    if (stage_in || stage_out) {
+        { int r = reserve(ctx, ctx->slot[1].h_in, ctx->max_chunks * (size_t)ENC_MAX_CHUNK); if (r) return r; }
+        { int r = reserve(ctx, ctx->slot[1].h_out, ctx->max_chunks * (size_t)kSlot); if (r) return r; }
     }
-    uint8_t *stg_in[2] = {ctx->h_in, ctx->h_in2}, *stg_out[2] = {ctx->h_out, ctx->h_out2};
     struct Pending { bool live; uint64_t pos, bytes; } pend[2] = {{false, 0, 0}, {false, 0, 0}};
     // a staged D2H copy of slot sl has landed in pinned memory: hand it to the caller's buffer
     auto drain = [&](int sl) -> int {
         if (!pend[sl].live) return B2C_OK;
-        if (cudaEventSynchronize(ctx->ev_out[sl]) != cudaSuccess) return B2C_ERR_CUDA;
-        parallel_memcpy((uint8_t *)h_dst + pend[sl].pos, stg_out[sl], pend[sl].bytes);
+        if (cudaEventSynchronize(ctx->slot[sl].ev_out) != cudaSuccess) return B2C_ERR_CUDA;
+        parallel_memcpy((uint8_t *)h_dst + pend[sl].pos, ctx->slot[sl].h_out.p, pend[sl].bytes);
         pend[sl].live = false;
         return B2C_OK;
     };
-    struct Slot { uint8_t *d_in, *d_out, *d_packed; int64_t *d_sizes, *h_sizes; uint64_t *d_off;
-                  uint32_t *d_ss, *h_ss; } slot[2] = {
-        {ctx->d_in, ctx->d_out, ctx->d_packed, ctx->d_sizes, ctx->h_sizes, ctx->d_offsets, ctx->d_src_sizes, ctx->h_src_sizes},
-        {ctx->d_in2, ctx->d_out2, ctx->d_packed2, ctx->d_sizes2, ctx->h_sizes2, ctx->d_offsets2, ctx->d_src_sizes2, ctx->h_src_sizes2}};
     uint64_t out_pos = 0;
     int rc = B2C_OK;
     // batch b's kernels are done: place its frames in the output stream and start the D2H copy
     auto finish = [&](size_t b) -> int {
         const int sl = (int)(b & 1);
-        Slot &S = slot[sl];
+        EncSlot &S = ctx->slot[sl];
         size_t c0 = bstart[b], m = bcount[b];
-        if (cudaEventSynchronize(ctx->ev[sl]) != cudaSuccess) return B2C_ERR_CUDA;
-        const int64_t *h_sz = S.h_sizes;
-        const uint64_t *h_off = reinterpret_cast<const uint64_t *>(S.h_sizes + m);
+        if (cudaEventSynchronize(S.ev) != cudaSuccess) return B2C_ERR_CUDA;
+        const int64_t *h_sz = S.h_sizes.p;
+        const uint64_t *h_off = reinterpret_cast<const uint64_t *>(h_sz + m);
         uint64_t total = h_off[m];
         if (out_pos + total > dst_cap) return B2C_ERR_DST_SMALL;
         if (stage_out) {
             { int rd = drain(sl); if (rd) return rd; }            // the slot's pinned buffer still holds batch b-2
-            if (cudaMemcpyAsync(stg_out[sl], S.d_packed, total, cudaMemcpyDeviceToHost, st_out) != cudaSuccess) return B2C_ERR_CUDA;
+            if (cudaMemcpyAsync(S.h_out.p, S.d_packed.p, total, cudaMemcpyDeviceToHost, st_out) != cudaSuccess) return B2C_ERR_CUDA;
             pend[sl].live = true; pend[sl].pos = out_pos; pend[sl].bytes = total;
-        } else if (cudaMemcpyAsync((uint8_t *)h_dst + out_pos, S.d_packed, total, cudaMemcpyDeviceToHost, st_out) != cudaSuccess)
+        } else if (cudaMemcpyAsync((uint8_t *)h_dst + out_pos, S.d_packed.p, total, cudaMemcpyDeviceToHost, st_out) != cudaSuccess)
             return B2C_ERR_CUDA;
-        if (cudaEventRecord(ctx->ev_out[sl], st_out) != cudaSuccess) return B2C_ERR_CUDA;
+        if (cudaEventRecord(S.ev_out, st_out) != cudaSuccess) return B2C_ERR_CUDA;
         if (stage_out) { int rd = drain(sl ^ 1); if (rd) return rd; }   // batch b-1's bytes have had a whole batch to arrive
         for (size_t i = 0; i < m; i++) {
             sizes_out[c0 + i] = h_sz[i];
@@ -928,27 +900,27 @@ static int encode_packed_impl(b2c_ctx *ctx, int level, int flags, const void *h_
     std::vector<const uint32_t *> bss(nb, nullptr);
     auto upload = [&](size_t b) -> int {
         const int sl = (int)(b & 1);
-        Slot &S = slot[sl];
+        EncSlot &S = ctx->slot[sl];
         size_t c0 = bstart[b], m = bcount[b];
         size_t off = c0 * (size_t)chunk_size;
         size_t bytes = (off + m * (size_t)chunk_size <= src_bytes) ? m * (size_t)chunk_size : src_bytes - off;
-        if (b >= 2) CK(cudaStreamWaitEvent(st_in, ctx->ev[sl], 0));
+        if (b >= 2) CK(cudaStreamWaitEvent(st_in, S.ev, 0));
         const uint8_t *from = (const uint8_t *)h_src + off;
         if (stage_in && bytes) {
-            if (b >= 2) CK(cudaEventSynchronize(ctx->ev_in[sl]));      // the H2D copy of batch b-2 has left the pinned buffer
-            parallel_memcpy(stg_in[sl], from, bytes);
-            from = stg_in[sl];
+            if (b >= 2) CK(cudaEventSynchronize(S.ev_in));      // the H2D copy of batch b-2 has left the pinned buffer
+            parallel_memcpy(S.h_in.p, from, bytes);
+            from = S.h_in.p;
         }
-        if (bytes) CK(cudaMemcpyAsync(S.d_in, from, bytes, cudaMemcpyHostToDevice, st_in));
+        if (bytes) CK(cudaMemcpyAsync(S.d_in.p, from, bytes, cudaMemcpyHostToDevice, st_in));
         if (bytes != m * (size_t)chunk_size) {  // ragged last chunk (or empty input): explicit sizes
             for (size_t i = 0; i < m; i++) {
                 size_t o = i * (size_t)chunk_size;
-                S.h_ss[i] = (uint32_t)(o >= bytes ? 0 : (bytes - o < chunk_size ? bytes - o : chunk_size));
+                S.h_src_sizes.p[i] = (uint32_t)(o >= bytes ? 0 : (bytes - o < chunk_size ? bytes - o : chunk_size));
             }
-            CK(cudaMemcpyAsync(S.d_ss, S.h_ss, m * sizeof(uint32_t), cudaMemcpyHostToDevice, st_in));
-            bss[b] = S.d_ss;
+            CK(cudaMemcpyAsync(S.d_src_sizes.p, S.h_src_sizes.p, m * sizeof(uint32_t), cudaMemcpyHostToDevice, st_in));
+            bss[b] = S.d_src_sizes.p;
         }
-        CK(cudaEventRecord(ctx->ev_in[sl], st_in));
+        CK(cudaEventRecord(S.ev_in, st_in));
         return B2C_OK;
     };
     // The copy of batch b+2 is queued before the host waits for batch b-1, so the H2D engine (the bottleneck) always
@@ -957,20 +929,20 @@ static int encode_packed_impl(b2c_ctx *ctx, int level, int flags, const void *h_
     if (nb > 1) { int r1 = upload(1); if (r1) return r1; }
     for (size_t b = 0; b < nb; b++) {
         const int sl = (int)(b & 1);
-        Slot &S = slot[sl];
+        EncSlot &S = ctx->slot[sl];
         size_t m = bcount[b];
         // kernels: need the input; the packed-output slot is free once batch b-2's D2H copy is done
-        CK(cudaStreamWaitEvent(st_c, ctx->ev_in[sl], 0));
-        if (b >= 2) CK(cudaStreamWaitEvent(st_c, ctx->ev_out[sl], 0));
-        int r = launch_encode(ctx, level, flags, S.d_in, chunk_size, bss[b], chunk_size, S.d_out, slotB, S.d_sizes,
+        CK(cudaStreamWaitEvent(st_c, S.ev_in, 0));
+        if (b >= 2) CK(cudaStreamWaitEvent(st_c, S.ev_out, 0));
+        int r = launch_encode(ctx, level, flags, S.d_in.p, chunk_size, bss[b], chunk_size, S.d_out.p, slotB, S.d_sizes.p,
                               (uint32_t)m, nullptr, nullptr, nullptr, 0, st_c, nullptr, sl);
         if (r) return r;
-        b2c_scan_sizes_kernel<<<1, 1024, 0, st_c>>>(S.d_sizes, S.d_off, (uint32_t)m);
-        b2c_pack_kernel<<<ctx->sm_count * 4, 256, 0, st_c>>>(S.d_out, slotB, S.d_sizes, S.d_off, S.d_packed, (uint32_t)m);
+        b2c_scan_sizes_kernel<<<1, 1024, 0, st_c>>>(S.d_sizes.p, S.d_offsets.p, (uint32_t)m);
+        b2c_pack_kernel<<<ctx->sm_count * 4, 256, 0, st_c>>>(S.d_out.p, slotB, S.d_sizes.p, S.d_offsets.p, S.d_packed.p, (uint32_t)m);
         ctx->launches += 2;
-        CK(cudaMemcpyAsync(S.h_sizes, S.d_sizes, m * sizeof(int64_t), cudaMemcpyDeviceToHost, st_c));
-        CK(cudaMemcpyAsync(S.h_sizes + m, S.d_off, (m + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st_c));
-        CK(cudaEventRecord(ctx->ev[sl], st_c));
+        CK(cudaMemcpyAsync(S.h_sizes.p, S.d_sizes.p, m * sizeof(int64_t), cudaMemcpyDeviceToHost, st_c));
+        CK(cudaMemcpyAsync(S.h_sizes.p + m, S.d_offsets.p, (m + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st_c));
+        CK(cudaEventRecord(S.ev, st_c));
         if (b + 2 < nb) { int r3 = upload(b + 2); if (r3) return r3; }
         if (b >= 1) { int r2 = finish(b - 1); if (r2) return r2; }
     }
@@ -999,26 +971,6 @@ int b2c_zstd_encode_packed(b2c_ctx *ctx, int level, int flags, const void *h_src
 }
 
 // ---- decoder ------------------------------------------------------------------------------------
-static int grow(b2c_ctx *ctx, uint8_t **p, size_t *cap, size_t need) {
-    if (*cap >= need) return B2C_OK;
-    CK(cudaDeviceSynchronize());
-    if (*p) CK(cudaFree(*p));
-    *p = nullptr; *cap = 0;
-    need += need / 4;
-    CK(cudaMalloc(p, need));
-    *cap = need;
-    return B2C_OK;
-}
-
-static int grow_host(b2c_ctx *ctx, uint8_t **p, size_t *cap, size_t need) {
-    if (*cap >= need) return B2C_OK;
-    if (*p) CK(cudaFreeHost(*p));
-    *p = nullptr; *cap = 0;
-    need += need / 4;
-    CK(cudaMallocHost(p, need));
-    *cap = need;
-    return B2C_OK;
-}
 // Pointer-table calls: n separately allocated host pieces <-> one packed device range.  Thousands of small
 // cudaMemcpyAsync calls cost more than the bytes they move (and block on pageable memory), so the pieces are gathered
 // into / scattered from one pinned staging buffer and cross the bus as ONE copy each way.  offs[i] = offset of piece i in
@@ -1032,13 +984,13 @@ static int gather_h2d(b2c_ctx *ctx, const void *const *srcs, const size_t *sizes
             if (sizes[i]) CK(cudaMemcpyAsync(d_base + offs[i], srcs[i], sizes[i], cudaMemcpyHostToDevice, st));
         return B2C_OK;
     }
-    int rc = grow_host(ctx, &ctx->h_stg_in, &ctx->h_stg_in_cap, total);
+    int rc = reserve(ctx, ctx->h_stg_in, total);
     if (rc) return rc;
     {
-        uint8_t *stg = ctx->h_stg_in;
+        uint8_t *stg = ctx->h_stg_in.p;
         parallel_pieces(n, total, [=](size_t i) { if (sizes[i]) memcpy(stg + offs[i], srcs[i], sizes[i]); });
     }
-    CK(cudaMemcpyAsync(d_base, ctx->h_stg_in, total, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_base, ctx->h_stg_in.p, total, cudaMemcpyHostToDevice, st));
     return B2C_OK;
 }
 // results: piece i = d_base[offs[i], offs[i] + lens[i]) -> dsts[i]; synchronises the stream
@@ -1053,30 +1005,55 @@ static int scatter_d2h(b2c_ctx *ctx, void *const *dsts, const size_t *lens, cons
         CK(cudaStreamSynchronize(st));
         return B2C_OK;
     }
-    int rc = grow_host(ctx, &ctx->h_stg_out, &ctx->h_stg_out_cap, range);
+    int rc = reserve(ctx, ctx->h_stg_out, range);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->h_stg_out, d_base, range, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(ctx->h_stg_out.p, d_base, range, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     {
-        const uint8_t *stg = ctx->h_stg_out;
+        const uint8_t *stg = ctx->h_stg_out.p;
         parallel_pieces(n, useful, [=](size_t i) { if (lens[i]) memcpy(dsts[i], stg + offs[i], lens[i]); });
     }
     return B2C_OK;
 }
 
+// Per-item arrays of the zstd and S2 host-buffer batches: filled on the host, copied to the device in one piece.
+struct BatchMeta {
+    struct Arrays { uint64_t *src_off, *dst_off; int64_t *res; uint32_t *src_sizes, *dst_caps; };
+    size_t off[5];
+    std::vector<uint8_t> host;
+    Arrays h;                                    // in `host`
+    explicit BatchMeta(size_t m) {
+        Layout L;
+        off[0] = L.take(sizeof(uint64_t) * m); off[1] = L.take(sizeof(uint64_t) * m); off[2] = L.take(sizeof(int64_t) * m);
+        off[3] = L.take(sizeof(uint32_t) * m); off[4] = L.take(sizeof(uint32_t) * m);
+        host.resize(L.end);
+        h = at(host.data());
+    }
+    Arrays at(uint8_t *base) const {
+        return {reinterpret_cast<uint64_t *>(base + off[0]), reinterpret_cast<uint64_t *>(base + off[1]),
+                reinterpret_cast<int64_t *>(base + off[2]), reinterpret_cast<uint32_t *>(base + off[3]),
+                reinterpret_cast<uint32_t *>(base + off[4])};
+    }
+};
+
 // lit_span: bytes of the output layout (literal areas mirror it: input c's area starts at c * lit_stride, or at
 // dst_offsets[c] when lit_stride is 0 -- the caller then guarantees non-overlapping, increasing offsets); 0 = unknown: the
 // one-warp decoder takes every input.
 static const uint64_t kStagedSpanLimit = 24ull << 30;
+// Grid of a one-warp decoder kernel over n inputs (DEC_WARPS per CTA): at most *max_grid CTAs, what the device holds at once.
+static unsigned dec_grid(const b2c_ctx *ctx, uint32_t n, unsigned *max_grid = nullptr) {
+    const unsigned ctasPerSm = (227u * 1024u) / (DEC_SMEM_BYTES + 1024u);
+    const unsigned grid = (n + DEC_WARPS - 1) / DEC_WARPS, maxGrid = (unsigned)ctx->sm_count * (ctasPerSm ? ctasPerSm : 1);
+    if (max_grid) *max_grid = maxGrid;
+    return grid < maxGrid ? grid : maxGrid;
+}
 static int launch_decode(b2c_ctx *ctx, ZstdDecParams &P, cudaStream_t st, uint64_t lit_span, uint64_t lit_stride) {
     if (P.nchunks == 0) return B2C_OK;
-    const unsigned ctasPerSm = (227u * 1024u) / (DEC_SMEM_BYTES + 1024u);
-    unsigned grid = (P.nchunks + DEC_WARPS - 1) / DEC_WARPS;
-    unsigned maxGrid = (unsigned)ctx->sm_count * (ctasPerSm ? ctasPerSm : 1);
-    if (grid > maxGrid) grid = maxGrid;
-    int rc = grow(ctx, &ctx->d_dec_lit, &ctx->dec_lit_cap, (size_t)maxGrid * DEC_WARPS * DEC_LIT_SCRATCH);
+    unsigned maxGrid;
+    const unsigned grid = dec_grid(ctx, P.nchunks, &maxGrid);
+    int rc = reserve(ctx, ctx->d_dec_lit, (size_t)maxGrid * DEC_WARPS * DEC_LIT_SCRATCH);
     if (rc) return rc;
-    P.lit_scratch = ctx->d_dec_lit;
+    P.lit_scratch = ctx->d_dec_lit.p;
     { int r = ctx_order_begin(ctx, st); if (r) return r; }    // the context's scratch is shared by all streams
     const uint32_t n = P.nchunks;
     const bool prof = ctx->dec_prof != 0;
@@ -1089,21 +1066,21 @@ static int launch_decode(b2c_ctx *ctx, ZstdDecParams &P, cudaStream_t st, uint64
     const bool staged = ctx->dec_staged && lit_span > 0 && lit_span <= kStagedSpanLimit && (uint64_t)n * maxb * FD_TAB_ENTRIES < (1ull << 31);
     ctx->fd_last = staged;
     if (staged) {
-        const size_t recBytes = (((size_t)n * sizeof(FdChunk)) + 255) & ~(size_t)255;
-        const size_t blkBytes = (((size_t)n * maxb * sizeof(FdBlock)) + 255) & ~(size_t)255;
-        const size_t tabBytes = (size_t)n * maxb * FD_TAB_ENTRIES * sizeof(uint32_t);
-        const size_t hufBytes = (size_t)n * maxb * 2048 * sizeof(uint16_t);
-        if ((rc = grow(ctx, &ctx->d_fd, &ctx->fd_cap, recBytes + blkBytes + tabBytes + hufBytes))) return rc;
-        if ((rc = grow(ctx, &ctx->d_fd_seq, &ctx->fd_seq_cap, 8 * ((size_t)(lit_span / 3) + 2 * (size_t)n + 8)))) return rc;
-        if ((rc = grow(ctx, &ctx->d_fd_lit, &ctx->fd_lit_cap, (size_t)lit_span + 64))) return rc;
-        P.fd = reinterpret_cast<FdChunk *>(ctx->d_fd);
-        P.fd_blk = reinterpret_cast<FdBlock *>(ctx->d_fd + recBytes);
+        Layout L;
+        const size_t oRec = L.take((size_t)n * sizeof(FdChunk)), oBlk = L.take((size_t)n * maxb * sizeof(FdBlock)),
+                     oTab = L.take((size_t)n * maxb * FD_TAB_ENTRIES * sizeof(uint32_t)),
+                     oHuf = L.take((size_t)n * maxb * 2048 * sizeof(uint16_t));
+        if ((rc = reserve(ctx, ctx->d_fd, L.end))) return rc;
+        if ((rc = reserve(ctx, ctx->d_fd_seq, 8 * ((size_t)(lit_span / 3) + 2 * (size_t)n + 8)))) return rc;
+        if ((rc = reserve(ctx, ctx->d_fd_lit, (size_t)lit_span + 64))) return rc;
+        P.fd = ctx->d_fd.at<FdChunk>(oRec);
+        P.fd_blk = ctx->d_fd.at<FdBlock>(oBlk);
         P.fd_maxb = maxb; P.fd_per_block = perBlock ? 1u : 0u;
-        P.fd_tabs = reinterpret_cast<uint32_t *>(ctx->d_fd + recBytes + blkBytes);
-        P.fd_huf = reinterpret_cast<uint16_t *>(ctx->d_fd + recBytes + blkBytes + tabBytes);
-        P.fd_const = ctx->d_fd_const;
-        P.fd_seqs = reinterpret_cast<uint64_t *>(ctx->d_fd_seq);
-        P.fd_lits = ctx->d_fd_lit;
+        P.fd_tabs = ctx->d_fd.at<uint32_t>(oTab);
+        P.fd_huf = ctx->d_fd.at<uint16_t>(oHuf);
+        P.fd_const = ctx->d_fd_const.p;
+        P.fd_seqs = ctx->d_fd_seq.at<uint64_t>(0);
+        P.fd_lits = ctx->d_fd_lit.p;
         P.fd_lit_stride = lit_stride;
         const uint32_t units = perBlock ? n * maxb : n;            // what the literal and sequence kernels spread over
         const unsigned groups = (units + FD_LIT_GROUP - 1) / FD_LIT_GROUP;
@@ -1271,27 +1248,24 @@ int b2c_zstd_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *
     first_item[n] = items.size();
     const size_t m = items.size();
     if (m > 0xffffffffull) return B2C_ERR_ARG;
-    // meta: src_off[m] u64 | dst_off[m] u64 | out_sizes[m] i64 | src_sizes[m] u32 | dst_caps[m] u32
-    std::vector<uint64_t> meta(3 * m + m);
-    uint64_t *so = meta.data(), *dof = so + m;
-    uint32_t *ss = reinterpret_cast<uint32_t *>(meta.data() + 3 * m), *dc = ss + m;
+    BatchMeta meta(m);
     for (size_t k = 0; k < m; k++) {
-        so[k] = in_base[items[k].input] + items[k].src_off_in_input;
-        dof[k] = out_base[items[k].input] + items[k].dst_off_in_input;
-        ss[k] = items[k].src_len; dc[k] = items[k].cap;
+        meta.h.src_off[k] = in_base[items[k].input] + items[k].src_off_in_input;
+        meta.h.dst_off[k] = out_base[items[k].input] + items[k].dst_off_in_input;
+        meta.h.src_sizes[k] = items[k].src_len; meta.h.dst_caps[k] = items[k].cap;
     }
     int rc;
-    if ((rc = grow(ctx, &ctx->d_dec_in, &ctx->dec_in_cap, inb + 64))) return rc;
-    if ((rc = grow(ctx, &ctx->d_dec_out, &ctx->dec_out_cap, outb + 64))) return rc;
-    if ((rc = grow(ctx, &ctx->d_dec_meta, &ctx->dec_meta_cap, meta.size() * 8))) return rc;
-    if ((rc = gather_h2d(ctx, srcs, src_sizes, in_base.data(), n, ctx->d_dec_in, (size_t)inb, st))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_dec_meta, meta.data(), meta.size() * 8, cudaMemcpyHostToDevice, st));
+    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 64))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 64))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_meta, meta.host.size()))) return rc;
+    if ((rc = gather_h2d(ctx, srcs, src_sizes, in_base.data(), n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
+    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, meta.host.data(), meta.host.size(), cudaMemcpyHostToDevice, st));
+    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p);
     ZstdDecParams P;
     memset(&P, 0, sizeof(P));
-    uint64_t *dm = reinterpret_cast<uint64_t *>(ctx->d_dec_meta);
-    P.src_base = ctx->d_dec_in; P.src_offsets = dm; P.src_sizes = reinterpret_cast<uint32_t *>(dm + 3 * m);
-    P.dst_base = ctx->d_dec_out; P.dst_offsets = dm + m; P.dst_caps = P.src_sizes + m;
-    P.out_sizes = reinterpret_cast<int64_t *>(dm + 2 * m); P.nchunks = (uint32_t)m;
+    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
+    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
+    P.out_sizes = d.res; P.nchunks = (uint32_t)m;
     if ((rc = launch_decode(ctx, P, st, outb, 0))) return rc;
     std::vector<int64_t> res(m);
     CK(cudaMemcpyAsync(res.data(), P.out_sizes, m * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -1314,7 +1288,7 @@ int b2c_zstd_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *
     {
         std::vector<size_t> lens(n);
         for (size_t i = 0; i < n; i++) lens[i] = (size_t)out_len[i];
-        if ((rc = scatter_d2h(ctx, dsts, lens.data(), out_base.data(), n, ctx->d_dec_out, (size_t)outb, st))) return rc;
+        if ((rc = scatter_d2h(ctx, dsts, lens.data(), out_base.data(), n, ctx->d_dec_out.p, (size_t)outb, st))) return rc;
     }
     return B2C_OK;
 }
@@ -1346,7 +1320,7 @@ static int launch_s2_encode(b2c_ctx *ctx, int level, int flags, const void *d_sr
     P.src_total = src_total;
     P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_cap = (uint32_t)dst_stride;
     P.out_sizes = d_out_sizes; P.nchunks = nchunks; P.blockmax = ENC_MAX_CHUNK;
-    P.scratch = ctx->d_scratch;
+    P.scratch = ctx->d_scratch.p;
     { int r = next_counter(ctx, st, &P.counter); if (r) return r; }
     const unsigned sms = (unsigned)ctx->sm_count;
     const bool snappy = (flags & B2C_S2_SNAPPY) != 0;
@@ -1395,20 +1369,13 @@ int b2c_s2_encode_stream_device(b2c_ctx *ctx, int level, int flags, const void *
     const uint32_t nblocks = (uint32_t)((n + block - 1) / block);
     const uint32_t sub = nblocks < 4096 ? (nblocks ? nblocks : 1) : 4096u, nsub = (nblocks + sub - 1) / sub;
     const size_t slotB = (b2c_s2_bound(block) + 15) & ~(size_t)15;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-    const size_t oSlots = take(slotB * sub), oEnc = take(sizeof(int64_t) * sub), oPiece = take(sizeof(int64_t) * sub),
-                 oCrc = take(sizeof(uint32_t) * sub), oScan = take(sizeof(uint64_t) * ((size_t)sub + 1)),
-                 oBase = take(sizeof(uint64_t) * ((size_t)nsub + 1));
-    if (ctx->s2s_cap < o) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->d_s2s) CK(cudaFree(ctx->d_s2s));
-        ctx->d_s2s = nullptr; ctx->s2s_cap = 0;
-        CK(cudaMalloc(&ctx->d_s2s, o));
-        ctx->s2s_cap = o;
-    }
+    Layout L;
+    const size_t oSlots = L.take(slotB * sub), oEnc = L.take(sizeof(int64_t) * sub), oPiece = L.take(sizeof(int64_t) * sub),
+                 oCrc = L.take(sizeof(uint32_t) * sub), oScan = L.take(sizeof(uint64_t) * ((size_t)sub + 1)),
+                 oBase = L.take(sizeof(uint64_t) * ((size_t)nsub + 1));
+    { int r = reserve(ctx, ctx->d_s2s, L.end); if (r) return r; }
     { int r = ctx_order_begin(ctx, st); if (r) return r; }
-    uint8_t *B = ctx->d_s2s;
+    uint8_t *B = ctx->d_s2s.p;
     uint64_t *d_base = (uint64_t *)(B + oBase);
     CK(cudaMemsetAsync(d_base, 0, sizeof(uint64_t), st));
     CK(cudaMemsetAsync(d_err, 0, sizeof(int32_t), st));
@@ -1450,17 +1417,12 @@ int b2c_s2_encode_stream(b2c_ctx *ctx, int level, int flags, const void *src, si
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     const size_t bound = b2c_s2_stream_bound(n, block);
-    const size_t inB = (n + 255) & ~(size_t)255, outB = (bound + 255) & ~(size_t)255;
-    if (ctx->s2s_io_cap < inB + outB + 512) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->d_s2s_io) CK(cudaFree(ctx->d_s2s_io));
-        ctx->d_s2s_io = nullptr; ctx->s2s_io_cap = 0;
-        CK(cudaMalloc(&ctx->d_s2s_io, inB + outB + 512));
-        ctx->s2s_io_cap = inB + outB + 512;
-    }
-    uint8_t *d_in = ctx->d_s2s_io, *d_out = d_in + inB;
-    uint64_t *d_total = (uint64_t *)(d_out + outB);
-    int32_t *d_err = (int32_t *)(d_total + 1);
+    Layout L;
+    const size_t oIn = L.take(n), oOut = L.take(bound), oTotal = L.take(sizeof(uint64_t)), oErr = L.take(sizeof(int32_t));
+    { int r = reserve(ctx, ctx->d_s2s_io, L.end); if (r) return r; }
+    uint8_t *d_in = ctx->d_s2s_io.at<uint8_t>(oIn), *d_out = ctx->d_s2s_io.at<uint8_t>(oOut);
+    uint64_t *d_total = ctx->d_s2s_io.at<uint64_t>(oTotal);
+    int32_t *d_err = ctx->d_s2s_io.at<int32_t>(oErr);
     if (n) CK(cudaMemcpyAsync(d_in, src, n, cudaMemcpyHostToDevice, st));
     int r = b2c_s2_encode_stream_device(ctx, level, flags, d_in, n, block, d_out, bound, d_total, d_err, st);
     if (r) { cudaStreamSynchronize(st); return r; }
@@ -1533,19 +1495,12 @@ int b2c_s2_decode_stream(b2c_ctx *ctx, const void *src, size_t n, void *dst, siz
     if (nb == 0) return B2C_OK;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t r = off; off += (bytes + 255) & ~(size_t)255; return r; };
-    const size_t oIn = take(n), oOut = take(total + 16), oBlk = take(sizeof(S2StreamBlock) * nb), oSrcOff = take(8 * (size_t)nb),
-                 oDstOff = take(8 * (size_t)nb), oSrcSz = take(4 * (size_t)nb), oCaps = take(4 * (size_t)nb),
-                 oRes = take(8 * (size_t)nb), oStat = take(4 * (size_t)nb);
-    if (ctx->s2s_io_cap < off) {
-        CK(cudaDeviceSynchronize());
-        if (ctx->d_s2s_io) CK(cudaFree(ctx->d_s2s_io));
-        ctx->d_s2s_io = nullptr; ctx->s2s_io_cap = 0;
-        CK(cudaMalloc(&ctx->d_s2s_io, off));
-        ctx->s2s_io_cap = off;
-    }
-    uint8_t *B = ctx->d_s2s_io;
+    Layout L;
+    const size_t oIn = L.take(n), oOut = L.take(total + 16), oBlk = L.take(sizeof(S2StreamBlock) * nb),
+                 oSrcOff = L.take(8 * (size_t)nb), oDstOff = L.take(8 * (size_t)nb), oSrcSz = L.take(4 * (size_t)nb),
+                 oCaps = L.take(4 * (size_t)nb), oRes = L.take(8 * (size_t)nb), oStat = L.take(4 * (size_t)nb);
+    { int r = reserve(ctx, ctx->d_s2s_io, L.end); if (r) return r; }
+    uint8_t *B = ctx->d_s2s_io.p;
     // compressed blocks go to the block decoder; an uncompressed chunk is handed to it as an empty job (size 0 in, cap 0)
     std::vector<uint64_t> so(nb), dof(nb);
     std::vector<uint32_t> ssz(nb), caps(nb);
@@ -1589,13 +1544,14 @@ static int launch_s2_decode(b2c_ctx *ctx, S2DecParams &P, uint64_t span, cudaStr
     const bool staged = ctx->dec_staged && span > 0 && span <= ((uint64_t)8 << 30);
     ctx->s2d_last = staged;
     if (staged) {
-        const size_t headBytes = (((size_t)n * sizeof(S2Head)) + 255) & ~(size_t)255;
+        Layout L;
         const size_t recBytes = ((size_t)(span / 3) + n + 16) * sizeof(uint64_t);
+        const size_t oHead = L.take((size_t)n * sizeof(S2Head)), oRec = L.take(recBytes);
         { int r = ctx_order_begin(ctx, st); if (r) return r; }
-        int rc = grow(ctx, &ctx->d_s2d, &ctx->s2d_cap, headBytes + recBytes);
+        int rc = reserve(ctx, ctx->d_s2d, oRec + recBytes);
         if (rc) return rc;
-        P.heads = reinterpret_cast<S2Head *>(ctx->d_s2d);
-        P.recs = reinterpret_cast<uint64_t *>(ctx->d_s2d + headBytes);
+        P.heads = ctx->d_s2d.at<S2Head>(oHead);
+        P.recs = ctx->d_s2d.at<uint64_t>(oRec);
         b2c_s2_walk_kernel<<<(n + 31) / 32, 32, 0, st>>>(P);
         b2c_s2_exec_kernel<<<(n + S2DEC_WARPS - 1) / S2DEC_WARPS, S2DEC_WARPS * 32, 0, st>>>(P);
         ctx->launches += 2;
@@ -1633,48 +1589,45 @@ static int s2_host_batch(b2c_ctx *ctx, bool encode, int level, int flags, const 
     if (n > 0xffffffffull) return B2C_ERR_ARG;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    std::vector<uint64_t> meta(3 * n + n);
-    uint64_t *so = meta.data(), *dof = so + n;
-    uint32_t *ss = reinterpret_cast<uint32_t *>(meta.data() + 3 * n), *dc = ss + n;
+    BatchMeta meta(n);
+    const BatchMeta::Arrays &h = meta.h;
     uint64_t inb = 0, outb = 0;
     for (size_t i = 0; i < n; i++) {
         if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
-        so[i] = inb; dof[i] = outb;
-        ss[i] = (uint32_t)src_sizes[i];
-        dc[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
+        h.src_off[i] = inb; h.dst_off[i] = outb;
+        h.src_sizes[i] = (uint32_t)src_sizes[i];
+        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
         // encode: fixed strides (the kernel addresses chunks by stride)
         inb += encode ? (size_t)ENC_MAX_CHUNK : ((src_sizes[i] + 15) & ~(size_t)15);
-        outb += encode ? (size_t)kSlot : (((size_t)dc[i] + 15) & ~(size_t)15);
+        outb += encode ? (size_t)kSlot : (((size_t)h.dst_caps[i] + 15) & ~(size_t)15);
     }
     int rc;
-    if ((rc = grow(ctx, &ctx->d_dec_in, &ctx->dec_in_cap, inb + 256))) return rc;
-    if ((rc = grow(ctx, &ctx->d_dec_out, &ctx->dec_out_cap, outb + 256))) return rc;
-    if ((rc = grow(ctx, &ctx->d_dec_meta, &ctx->dec_meta_cap, meta.size() * 8))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_meta, meta.host.size()))) return rc;
     {
         std::vector<size_t> lens(n);
         for (size_t i = 0; i < n; i++) {
             lens[i] = src_sizes[i];
-            if (encode && src_sizes[i] > ENC_MAX_CHUNK) { ss[i] = ENC_MAX_CHUNK + 1; lens[i] = 0; }   // reported as too big
+            if (encode && src_sizes[i] > ENC_MAX_CHUNK) { h.src_sizes[i] = ENC_MAX_CHUNK + 1; lens[i] = 0; }   // reported as too big
         }
-        if ((rc = gather_h2d(ctx, srcs, lens.data(), so, n, ctx->d_dec_in, (size_t)inb, st))) return rc;
+        if ((rc = gather_h2d(ctx, srcs, lens.data(), h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
     }
-    CK(cudaMemcpyAsync(ctx->d_dec_meta, meta.data(), meta.size() * 8, cudaMemcpyHostToDevice, st));
-    uint64_t *dm = reinterpret_cast<uint64_t *>(ctx->d_dec_meta);
-    uint32_t *d_ss = reinterpret_cast<uint32_t *>(dm + 3 * n);
-    int64_t *d_res = reinterpret_cast<int64_t *>(dm + 2 * n);
+    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, meta.host.data(), meta.host.size(), cudaMemcpyHostToDevice, st));
+    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p);
     if (encode)
-        rc = b2c_s2_encode_device(ctx, level, flags, ctx->d_dec_in, ENC_MAX_CHUNK, d_ss, 0, ctx->d_dec_out, kSlot, d_res,
+        rc = b2c_s2_encode_device(ctx, level, flags, ctx->d_dec_in.p, ENC_MAX_CHUNK, d.src_sizes, 0, ctx->d_dec_out.p, kSlot, d.res,
                                   (uint32_t)n, st);
     else {
         S2DecParams P;
         memset(&P, 0, sizeof(P));
-        P.src_base = ctx->d_dec_in; P.src_offsets = dm; P.src_sizes = d_ss;
-        P.dst_base = ctx->d_dec_out; P.dst_offsets = dm + n; P.dst_caps = d_ss + n;
-        P.out_sizes = d_res; P.nchunks = (uint32_t)n;
+        P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
+        P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
+        P.out_sizes = d.res; P.nchunks = (uint32_t)n;
         rc = launch_s2_decode(ctx, P, inb, st);
     }
     if (rc) return rc;
-    CK(cudaMemcpyAsync(sizes_out, d_res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     {
         std::vector<size_t> lens(n, 0);
@@ -1682,7 +1635,7 @@ static int s2_host_batch(b2c_ctx *ctx, bool encode, int level, int flags, const 
             if (sizes_out[i] > 0 && (size_t)sizes_out[i] > dst_caps[i]) { sizes_out[i] = B2C_ERR_DST_SMALL; continue; }
             if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
         }
-        if ((rc = scatter_d2h(ctx, dsts, lens.data(), dof, n, ctx->d_dec_out, (size_t)outb, st))) return rc;
+        if ((rc = scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st))) return rc;
     }
     return B2C_OK;
 }
@@ -1730,23 +1683,22 @@ int b2c_huf_decompress_device(b2c_ctx *ctx, int flags, const void *d_src, size_t
     P.src_base = (const uint8_t *)d_src; P.src_stride = src_stride; P.src_sizes = d_src_sizes;
     P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_sizes = d_dst_sizes;
     P.out_sizes = d_out_sizes; P.nchunks = nchunks; P.flags = (flags & B2C_HUF_4X) ? HUF0_FLAG_4X : 0;
-    const unsigned ctasPerSm = (227u * 1024u) / (DEC_SMEM_BYTES + 1024u);
-    unsigned grid = (nchunks + DEC_WARPS - 1) / DEC_WARPS, maxGrid = (unsigned)ctx->sm_count * (ctasPerSm ? ctasPerSm : 1);
-    if (grid > maxGrid) grid = maxGrid;
+    const unsigned grid = dec_grid(ctx, nchunks);
     cudaStream_t st = (cudaStream_t)stream;
     // Staged form (the default): table pass -> the staged zstd decoder's literal-stream kernel -> the one-warp kernel over what
     // is left (errors, unusual blocks).  B2C_DEC=onewarp, very large batches and unaligned slots keep the one-warp kernel alone.
     const bool staged = ctx->dec_staged && nchunks <= (1u << 20) && (dst_stride & 3) == 0;
     if (staged) {
-        const size_t recBytes = (((size_t)nchunks * sizeof(FdChunk)) + 255) & ~(size_t)255;
-        const size_t blkBytes = (((size_t)nchunks * sizeof(FdBlock)) + 255) & ~(size_t)255;
-        const size_t hufBytes = (size_t)nchunks * 2048 * sizeof(uint16_t);
+        ctx->fd_last = false;           // the records below overwrite the zstd decoder's
+        Layout L;
+        const size_t oRec = L.take((size_t)nchunks * sizeof(FdChunk)), oBlk = L.take((size_t)nchunks * sizeof(FdBlock)),
+                     oHuf = L.take((size_t)nchunks * 2048 * sizeof(uint16_t));
         { int r = ctx_order_begin(ctx, st); if (r) return r; }
-        int rc = grow(ctx, &ctx->d_fd, &ctx->fd_cap, recBytes + blkBytes + hufBytes);
+        int rc = reserve(ctx, ctx->d_fd, L.end);
         if (rc) return rc;
-        P.fd = reinterpret_cast<FdChunk *>(ctx->d_fd);
-        P.fd_blk = reinterpret_cast<FdBlock *>(ctx->d_fd + recBytes);
-        P.fd_huf = reinterpret_cast<uint16_t *>(ctx->d_fd + recBytes + blkBytes);
+        P.fd = ctx->d_fd.at<FdChunk>(oRec);
+        P.fd_blk = ctx->d_fd.at<FdBlock>(oBlk);
+        P.fd_huf = ctx->d_fd.at<uint16_t>(oHuf);
         b2c_huf_dec_prep_kernel<<<grid, DEC_WARPS * 32, DEC_SMEM_BYTES, st>>>(P);
         ZstdDecParams Z;
         memset(&Z, 0, sizeof(Z));
@@ -1789,28 +1741,25 @@ static int huf_host_batch(b2c_ctx *ctx, int op, int flags, const void *const *sr
     uint32_t *ss = reinterpret_cast<uint32_t *>(meta.data() + n), *ds = ss + n;
     for (size_t i = 0; i < n; i++) { ss[i] = (uint32_t)src_sizes[i]; ds[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]); }
     int rc;
-    if ((rc = grow(ctx, &ctx->d_dec_in, &ctx->dec_in_cap, n * inStride + 256))) return rc;
-    if ((rc = grow(ctx, &ctx->d_dec_out, &ctx->dec_out_cap, n * outStride + 256))) return rc;
-    if ((rc = grow(ctx, &ctx->d_dec_meta, &ctx->dec_meta_cap, meta.size() * 8))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_in, n * inStride + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_out, n * outStride + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_meta, meta.size() * 8))) return rc;
     for (size_t i = 0; i < n; i++)
-        if (src_sizes[i]) CK(cudaMemcpyAsync(ctx->d_dec_in + i * inStride, srcs[i], src_sizes[i], cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(ctx->d_dec_meta, meta.data(), meta.size() * 8, cudaMemcpyHostToDevice, st));
-    uint64_t *dm = reinterpret_cast<uint64_t *>(ctx->d_dec_meta);
+        if (src_sizes[i]) CK(cudaMemcpyAsync(ctx->d_dec_in.p + i * inStride, srcs[i], src_sizes[i], cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, meta.data(), meta.size() * 8, cudaMemcpyHostToDevice, st));
+    uint64_t *dm = ctx->d_dec_meta.at<uint64_t>(0);
     int64_t *d_res = reinterpret_cast<int64_t *>(dm);
     uint32_t *d_ss = reinterpret_cast<uint32_t *>(dm + n), *d_ds = d_ss + n;
     if (op == 0)
-        rc = b2c_huf_compress_device(ctx, flags, ctx->d_dec_in, inStride, d_ss, 0, ctx->d_dec_out, outStride, d_res, (uint32_t)n, st);
+        rc = b2c_huf_compress_device(ctx, flags, ctx->d_dec_in.p, inStride, d_ss, 0, ctx->d_dec_out.p, outStride, d_res, (uint32_t)n, st);
     else if (op == 1)
-        rc = b2c_huf_decompress_device(ctx, flags, ctx->d_dec_in, inStride, d_ss, ctx->d_dec_out, outStride, d_ds, d_res, (uint32_t)n, st);
+        rc = b2c_huf_decompress_device(ctx, flags, ctx->d_dec_in.p, inStride, d_ss, ctx->d_dec_out.p, outStride, d_ds, d_res, (uint32_t)n, st);
     else {
         Huf0Params P;
         memset(&P, 0, sizeof(P));
-        P.src_base = ctx->d_dec_in; P.src_stride = inStride; P.src_sizes = d_ss;
-        P.dst_base = ctx->d_dec_out; P.dst_stride = outStride; P.out_sizes = d_res; P.nchunks = (uint32_t)n;
-        const unsigned ctasPerSm = (227u * 1024u) / (DEC_SMEM_BYTES + 1024u);
-        unsigned grid = ((unsigned)n + DEC_WARPS - 1) / DEC_WARPS, maxGrid = (unsigned)ctx->sm_count * (ctasPerSm ? ctasPerSm : 1);
-        if (grid > maxGrid) grid = maxGrid;
-        b2c_huf_read_table_kernel<<<grid, DEC_WARPS * 32, DEC_SMEM_BYTES, st>>>(P);
+        P.src_base = ctx->d_dec_in.p; P.src_stride = inStride; P.src_sizes = d_ss;
+        P.dst_base = ctx->d_dec_out.p; P.dst_stride = outStride; P.out_sizes = d_res; P.nchunks = (uint32_t)n;
+        b2c_huf_read_table_kernel<<<dec_grid(ctx, (uint32_t)n), DEC_WARPS * 32, DEC_SMEM_BYTES, st>>>(P);
         ctx->launches += 1;
         CK(cudaGetLastError());
         rc = B2C_OK;
@@ -1822,7 +1771,7 @@ static int huf_host_batch(b2c_ctx *ctx, int op, int flags, const void *const *sr
         if (sizes_out[i] < 0) continue;
         const size_t bytes = op == 2 ? 260 : (size_t)sizes_out[i];
         if (op == 0 && bytes > dst_caps[i]) { sizes_out[i] = B2C_ERR_DST_SMALL; continue; }
-        if (bytes) CK(cudaMemcpyAsync(dsts[i], ctx->d_dec_out + i * outStride, bytes, cudaMemcpyDeviceToHost, st));
+        if (bytes) CK(cudaMemcpyAsync(dsts[i], ctx->d_dec_out.p + i * outStride, bytes, cudaMemcpyDeviceToHost, st));
     }
     CK(cudaStreamSynchronize(st));
     return B2C_OK;

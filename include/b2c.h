@@ -92,7 +92,9 @@ B2C_API int b2c_decode_profile_read(b2c_ctx *ctx, double *ms);
  * rest were decoded by the one-warp decoder).  Synchronises the device. */
 B2C_API int b2c_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged);
 B2C_API int b2c_s2_decode_staged_count(b2c_ctx *ctx, uint32_t nchunks, uint32_t *staged);   /* the same for S2 block decode */
-/* test hooks: per input, flags[i] = 1 if the staged kernels completed input i of the most recent (S2) decode launch, else 0 */
+/* test hooks: per input, flags[i] = 1 if the staged kernels completed input i of the most recent (S2) decode launch, else 0.
+ * Every flag is 0 when that launch did not run the staged kernels, and after a staged huff0 decompress (which reuses the
+ * zstd decoder's per-input records). */
 B2C_API int b2c_decode_staged_flags(b2c_ctx *ctx, uint32_t nchunks, uint8_t *flags);
 B2C_API int b2c_s2_decode_staged_flags(b2c_ctx *ctx, uint32_t nchunks, uint8_t *flags);
 
