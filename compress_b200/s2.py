@@ -41,6 +41,10 @@ class ErrTooLarge(B2CError):
     pass
 
 
+class ErrDstTooSmall(B2CError):
+    """s2.ErrDstTooSmall (s2/lz4convert.go:19)"""
+
+
 def MaxEncodedLen(n):
     r = int(lib.b2c_s2_bound(n))
     return r if (r or n == 0) and n <= 0xffffffff else -1
@@ -216,6 +220,49 @@ class Codec:
         if codes[0] < 0:
             raise ErrCorrupt("s2: corrupt input")
         return outs[0]
+
+    # ---- LZ4 / LZ4s -> S2 / Snappy blocks (s2.LZ4Converter / s2.LZ4sConverter, s2/lz4convert.go, s2/lz4sconvert.go) ----
+    def convert_lz4_blocks(self, blocks, caps, lz4s=False, snappy=False):
+        """Convert LZ4 (or LZ4s) blocks; caps[i] = slot capacity.  Returns (outs, codes, ns): outs[i] = uvarint(n) + the S2
+        (Snappy) body or None, codes[i] = its size or a negative error, ns[i] = the decoded size."""
+        n = len(blocks)
+        if n == 0:
+            return [], [], []
+        bufs = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(1, dtype=np.uint8) for b in blocks]
+        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
+        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
+        ssz = (ctypes.c_size_t * n)(*[len(b) for b in blocks])
+        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
+        dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
+        res, dec = (ctypes.c_int64 * n)(), (ctypes.c_int64 * n)()
+        check(lib.b2c_s2_convert_lz4_chunks(self._ctx, 1 if lz4s else 0, FLAG_SNAPPY if snappy else 0, srcs, ssz, dsts, dcap,
+                                            res, dec, n), self._ctx)
+        codes = [int(r) for r in res]
+        return [outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes, [int(x) for x in dec]
+
+    def convert_lz4_device(self, src, src_sizes, src_stride, lz4s=False, snappy=False, dst=None, dst_cap=None, out_sizes=None,
+                           decoded=None, src_offsets=None, dst_offsets=None, dst_stride=None):
+        """src: uint8 CUDA tensor, block i at i * src_stride (or src_offsets[i]; then every block is at most src_stride bytes).
+        Slot i at i * dst_stride (or dst_offsets[i]) with dst_cap bytes.  Returns (dst, out_sizes int64, decoded int64).  Async."""
+        assert src.is_cuda and src.dtype == torch.uint8
+        n = src_sizes.numel()
+        if dst_cap is None:
+            dst_cap = src_stride + src_stride // 2 + 64
+        if dst_stride is None:
+            dst_stride = dst_cap
+        if dst is None:
+            dst = torch.empty((n, dst_stride), dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty((n,), dtype=torch.int64, device=src.device)
+        if decoded is None:
+            decoded = torch.empty((n,), dtype=torch.int64, device=src.device)
+        stream = torch.cuda.current_stream(src.device).cuda_stream
+        check(lib.b2c_s2_convert_lz4_device(self._ctx, 1 if lz4s else 0, FLAG_SNAPPY if snappy else 0, src.data_ptr(), src_stride,
+                                            None if src_offsets is None else src_offsets.data_ptr(), src_sizes.data_ptr(),
+                                            dst.data_ptr(), dst_stride, None if dst_offsets is None else dst_offsets.data_ptr(),
+                                            dst_cap, out_sizes.data_ptr(), decoded.data_ptr(), n, ctypes.c_void_p(stream)),
+              self._ctx)
+        return dst, out_sizes, decoded
 
     # ---- streams: the framing format (s2.Writer.EncodeBuffer / s2.Reader, s2/writer.go:357-470, s2/reader.go:249-420) ----
     def EncodeStream(self, src, better=False, snappy=False, block_size=BLOCK, index=False):
@@ -693,3 +740,44 @@ class ReadSeeker:
                 break
             out += part
         return bytes(out)
+
+
+# ---- LZ4 / LZ4s converters (s2/lz4convert.go:13-275, s2/lz4sconvert.go:23-284) ---------------------------------------------
+class LZ4Converter:
+    """s2.LZ4Converter on the device.  ConvertBlock(dst, src, cap) appends the S2 form of the LZ4 block src to dst, where cap is
+    the Go slice's capacity (cap(dst) >= len(dst)); returns (dst + body, decoded size) or raises ErrCorrupt / ErrDstTooSmall
+    as the reference does (ErrTooLarge for a decoded size above 2^32 - 1).  ConvertBlockSnappy writes Snappy instead."""
+    _lz4s = False
+
+    def __init__(self, codec=None, device=0):
+        self._codec = codec if codec is not None else Codec(device=device)
+
+    def _convert(self, dst, src, cap, snappy):
+        dst = bytes(dst)
+        if cap is None:
+            cap = len(dst)
+        if cap < len(dst):
+            raise ValueError("cap below len(dst)")
+        if len(src) == 0:
+            return dst, 0
+        outs, codes, ns = self._codec.convert_lz4_blocks([src], [cap - len(dst) + 5], lz4s=self._lz4s, snappy=snappy)
+        if codes[0] == -5:
+            raise ErrCorrupt("s2: corrupt input")
+        if codes[0] == -4:
+            raise ErrDstTooSmall("s2: destination too small")
+        if codes[0] == -3:
+            raise ErrTooLarge("s2: decoded block is too large")
+        if codes[0] < 0:
+            raise B2CError(lib.b2c_strerror(codes[0]).decode())
+        return dst + outs[0][_decoded_len(outs[0])[1]:], ns[0]
+
+    def ConvertBlock(self, dst, src, cap=None):
+        return self._convert(dst, src, cap, False)
+
+    def ConvertBlockSnappy(self, dst, src, cap=None):
+        return self._convert(dst, src, cap, True)
+
+
+class LZ4sConverter(LZ4Converter):
+    """s2.LZ4sConverter: the same for LZ4s blocks (Intel QAT's LZ4 variant, where a match length of 3 means no match)."""
+    _lz4s = True

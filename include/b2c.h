@@ -207,6 +207,30 @@ B2C_API int b2c_s2_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const si
                                  const size_t *dst_caps, int64_t *sizes_out, size_t n);
 
 /*
+ * LZ4 / LZ4s block -> S2 / Snappy block (s2.LZ4Converter / s2.LZ4sConverter ConvertBlock and ConvertBlockSnappy,
+ * s2/lz4convert.go:25,281, s2/lz4sconvert.go:30,290): the token stream is rewritten without decompressing.  format:
+ * B2C_LZ4 or B2C_LZ4S (the LZ4 variant Intel QAT emits: a match length of 3 means "no match"); flags: B2C_S2_SNAPPY for
+ * ConvertBlockSnappy.  Slot i receives uvarint(n) followed by the bytes ConvertBlock* appends, so it is a complete block
+ * s2.Decode reads; sizes_out[i] = its bytes, decoded[i] = n.  The outcome is the reference's for a dst with
+ * cap(dst) - len(dst) = slot capacity - 5: B2C_ERR_CORRUPT (ErrCorrupt) or B2C_ERR_DST_SMALL (ErrDstTooSmall), also where
+ * the reference's inlined S2 emitters would write past cap(dst) (they only check for 5 bytes of room).  A decoded size
+ * above 2^32 - 1 cannot be stated in an S2 header: B2C_ERR_TOO_BIG, decoded[i] = n.  decoded[i] = 0 for the other errors.
+ * _device: argument conventions of b2c_s2_decode_device, asynchronous on `stream`.  Without d_src_offsets block i is at
+ * d_src + i * src_stride; with them src_stride is the bound on every block's size.  A block larger than src_stride is
+ * B2C_ERR_ARG.  Scratch for up to (src_stride / 3 + 1) 16-byte records per block (LZ4S: / 2) is held by the context; a call
+ * needing more than 4 GiB of it runs in passes.
+ * _chunks: host buffers, synchronous.
+ */
+enum { B2C_LZ4 = 0, B2C_LZ4S = 1 };
+B2C_API int b2c_s2_convert_lz4_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                                      const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, void *d_dst,
+                                      size_t dst_stride, const uint64_t *d_dst_offsets, uint32_t dst_cap,
+                                      int64_t *d_out_sizes, int64_t *d_decoded, uint32_t nchunks, void *stream);
+B2C_API int b2c_s2_convert_lz4_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                                      void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, int64_t *decoded,
+                                      size_t n);
+
+/*
  * S2 / Snappy STREAMS (the framing format: s2.Writer.EncodeBuffer, s2/writer.go:357-470, and s2.Reader over a buffer,
  * s2/reader.go:249-420; constants and the masked CRC32-C: s2/s2.go:75-126).  A stream = the identifier chunk, then per
  * block (<= 64 KiB here, WriterBlockSize) one chunk: type (0 compressed, 1 uncompressed), 24-bit length, checksum of the
