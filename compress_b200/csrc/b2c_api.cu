@@ -87,6 +87,7 @@ struct b2c_ctx {
     Buf<> d_fr_io{kDevice, kExact};     // frame mode, host-buffer call: staged input | packed output | results
     Buf<> d_s2d{kDevice, kHeadroom};    // staged S2 block decode: block heads + element records
     Buf<> d_lzc{kDevice, kHeadroom};    // LZ4 -> S2 conversion: block heads + sequence records of one pass
+    Buf<> d_s2best{kDevice, kExact};    // S2 best parse scratch (four candidates per position), reserved on first use
     Buf<> d_s2s{kDevice, kExact};       // S2 stream calls: block slots, sizes, checksums, scan, tables (grown on demand)
     Buf<> d_s2s_io{kDevice, kExact};    //   host-buffer calls: staged input | output
     Buf<uint32_t> d_counters{kDevice, kExact}; uint32_t counter_seq = 0;   // chunk counters of the persistent parse kernels (one per launch, rotating)
@@ -258,6 +259,8 @@ b2c_ctx *b2c_ctx_create(int device, size_t max_chunks) {
         {(const void *)b2c_lz_snappy_fast_kernel, (int)LzLayout<3>::SMEM_BYTES},
         {(const void *)b2c_lz_s2_better_kernel, (int)LzLayout<4>::SMEM_BYTES},
         {(const void *)b2c_lz_snappy_better_kernel, (int)LzLayout<4>::SMEM_BYTES},
+        {(const void *)b2c_lz_s2_best_kernel, (int)LzLayout<LZ_S2BEST>::SMEM_BYTES},
+        {(const void *)b2c_lz_snappy_best_kernel, (int)LzLayout<LZ_S2BEST>::SMEM_BYTES},
         {(const void *)b2c_zstd_hist_kernel, (int)HIST_SMEM_BYTES},
         {(const void *)b2c_zstd_pack128_kernel, (int)PackCfg<131072>::SMEM_BYTES},
         {(const void *)b2c_zstd_pack_kernel, (int)PACK_SMEM_BYTES},
@@ -1311,7 +1314,7 @@ static int launch_s2_encode(b2c_ctx *ctx, int level, int flags, const void *d_sr
                             const uint32_t *d_sizes, uint32_t size_all, uint64_t src_total, void *d_dst, size_t dst_stride,
                             int64_t *d_out_sizes, uint32_t nchunks, cudaStream_t st) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
-    if (level != B2C_S2_FAST && level != B2C_S2_BETTER) return B2C_ERR_UNSUPPORTED;
+    if (level != B2C_S2_FAST && level != B2C_S2_BETTER && level != B2C_S2_BEST) return B2C_ERR_UNSUPPORTED;
     if (nchunks == 0) return B2C_OK;
     if (dst_stride > 0xffffffffull) return B2C_ERR_ARG;
     CK(cudaSetDevice(ctx->device));
@@ -1323,6 +1326,11 @@ static int launch_s2_encode(b2c_ctx *ctx, int level, int flags, const void *d_sr
     P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_cap = (uint32_t)dst_stride;
     P.out_sizes = d_out_sizes; P.nchunks = nchunks; P.blockmax = ENC_MAX_CHUNK;
     P.scratch = ctx->d_scratch.p;
+    if (level == B2C_S2_BEST) {     // (its own scratch: four candidate distances per position do not fit the shared set)
+        const size_t need = (size_t)ctx->sm_count * LzCfg<LZ_S2BEST>::MIN_CTAS * LzLayout<LZ_S2BEST>::SCRATCH_BYTES;
+        { int r = reserve(ctx, ctx->d_s2best, need); if (r) return r; }
+        P.scratch = ctx->d_s2best.p;
+    }
     { int r = next_counter(ctx, st, &P.counter); if (r) return r; }
     const unsigned sms = (unsigned)ctx->sm_count;
     const bool snappy = (flags & B2C_S2_SNAPPY) != 0;
@@ -1330,10 +1338,14 @@ static int launch_s2_encode(b2c_ctx *ctx, int level, int flags, const void *d_sr
         const unsigned cap = sms * LzCfg<3>::MIN_CTAS, g1 = cap < nchunks ? cap : nchunks;
         if (snappy) b2c_lz_snappy_fast_kernel<<<g1, LzCfg<3>::NT, LzLayout<3>::SMEM_BYTES, st>>>(P);
         else b2c_lz_s2_fast_kernel<<<g1, LzCfg<3>::NT, LzLayout<3>::SMEM_BYTES, st>>>(P);
-    } else {
+    } else if (level == B2C_S2_BETTER) {
         const unsigned cap = sms * LzCfg<4>::MIN_CTAS, g1 = cap < nchunks ? cap : nchunks;
         if (snappy) b2c_lz_snappy_better_kernel<<<g1, LzCfg<4>::NT, LzLayout<4>::SMEM_BYTES, st>>>(P);
         else b2c_lz_s2_better_kernel<<<g1, LzCfg<4>::NT, LzLayout<4>::SMEM_BYTES, st>>>(P);
+    } else {
+        const unsigned cap = sms * LzCfg<LZ_S2BEST>::MIN_CTAS, g1 = cap < nchunks ? cap : nchunks;
+        if (snappy) b2c_lz_snappy_best_kernel<<<g1, LzCfg<LZ_S2BEST>::NT, LzLayout<LZ_S2BEST>::SMEM_BYTES, st>>>(P);
+        else b2c_lz_s2_best_kernel<<<g1, LzCfg<LZ_S2BEST>::NT, LzLayout<LZ_S2BEST>::SMEM_BYTES, st>>>(P);
     }
     ctx->launches += 1;
     CK(cudaGetLastError());
@@ -1363,7 +1375,7 @@ size_t b2c_s2_stream_bound(size_t n, size_t block) {
 int b2c_s2_encode_stream_device(b2c_ctx *ctx, int level, int flags, const void *d_src, uint64_t n, uint32_t block, void *d_dst,
                                 uint64_t dst_cap, uint64_t *d_total, int32_t *d_err, void *stream) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
-    if (level != B2C_S2_FAST && level != B2C_S2_BETTER) return B2C_ERR_UNSUPPORTED;
+    if (level != B2C_S2_FAST && level != B2C_S2_BETTER && level != B2C_S2_BEST) return B2C_ERR_UNSUPPORTED;
     if (block == 0 || block > 65536 || !d_total || !d_err) return B2C_ERR_ARG;
     if (n / block >= 0x7fffffffull || dst_cap < 10) return B2C_ERR_ARG;
     CK(cudaSetDevice(ctx->device));
@@ -1644,7 +1656,7 @@ static int s2_host_batch(b2c_ctx *ctx, bool encode, int level, int flags, const 
 
 int b2c_s2_encode_chunks(b2c_ctx *ctx, int level, int flags, const void *const *srcs, const size_t *src_sizes,
                          void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, size_t n) {
-    if (level != B2C_S2_FAST && level != B2C_S2_BETTER) return ctx ? B2C_ERR_UNSUPPORTED : B2C_ERR_NO_DEVICE;
+    if (level != B2C_S2_FAST && level != B2C_S2_BETTER && level != B2C_S2_BEST) return ctx ? B2C_ERR_UNSUPPORTED : B2C_ERR_NO_DEVICE;
     return s2_host_batch(ctx, true, level, flags, srcs, src_sizes, dsts, dst_caps, sizes_out, n);
 }
 int b2c_s2_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *src_sizes, void *const *dsts,

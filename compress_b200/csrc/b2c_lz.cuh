@@ -117,32 +117,57 @@ template <> struct LzCfg<4> {
     static constexpr uint32_t KREC = 12;      // (the second bitmap takes the room of four records per thread)
     static constexpr int MIN_CTAS = 2;
 };
+// S2 best (s2/encode_best.go:22-716 encodeBlockBest / encodeBlockBestSnappy: long 8-byte + short 4-byte table, two
+// positions per slot, cost-scored choice among the candidates at s, s+1, s+2, the repeat and the match end): the better
+// shape, but the dense pass keeps four candidates per position (near and far of both tables) and the walk scores them
+// (lz_walk_best).  Larger tables than any other class -- 2^15 short and 2^14 long slots, 192 KiB -- because most of what
+// the serial encoder gains over better comes from finding the earlier occurrences of short strings (measured under the
+// emulator: with 2^13 slots in both tables the output was 4-7 % larger on text and digits).  They fit one CTA per SM;
+// the match records and per-thread arrays, which live only after the dense pass, share the dead tables' memory.
+enum { LZ_S2BEST = 6 };
+constexpr uint32_t LZ_BEST_LBITS = 14;      // long table of the best class (its short table: LzCfg<6>::TBITS)
+template <> struct LzCfg<6> {
+    static constexpr int NT = 512;
+    static constexpr uint32_t BLOCK = 65536;
+    static constexpr bool LONG = true;
+    static constexpr int SMLS = 4, LMLS = 8;
+    static constexpr int PPT = 1;
+    static constexpr int INS = 1;
+    static constexpr uint32_t TBITS = 15;
+    static constexpr uint32_t KREC = 12;
+    static constexpr int MIN_CTAS = 1;
+};
 
 template <int LV> struct LzLayout {
     using C = LzCfg<LV>;
     static constexpr uint32_t NTAB = C::LONG ? 2 : 1;
-    static constexpr uint32_t TAB_BYTES = NTAB * (4u << C::TBITS);
+    static constexpr bool BEST = LV == LZ_S2BEST;
+    static constexpr uint32_t TAB_BYTES = BEST ? (4u << C::TBITS) + (4u << LZ_BEST_LBITS) : NTAB * (4u << C::TBITS);
     static constexpr uint32_t SRC_BYTES = C::BLOCK + 128;
     static constexpr uint32_t A_BYTES = TAB_BYTES > SRC_BYTES ? TAB_BYTES : SRC_BYTES;
     static constexpr uint32_t BM_BYTES = C::BLOCK / 8 + 16;
     static constexpr uint32_t SM_A = 0;
     static constexpr uint32_t SM_BM = SM_A + A_BYTES;
     static constexpr uint32_t SM_BML = SM_BM + BM_BYTES;
-    static constexpr uint32_t SM_REC = SM_BML + (C::LONG ? BM_BYTES : 0);
+    // (best: the records and the arrays follow the staged chunk inside the dead tables)
+    static constexpr uint32_t SM_REC = BEST ? (SRC_BYTES + 15) / 16 * 16 : SM_BML + (C::LONG ? BM_BYTES : 0);
     static constexpr uint32_t REC_BYTES = C::KREC * C::NT * 4;
     static constexpr uint32_t SM_ARR = SM_REC + REC_BYTES;                      // keptEnd u32 | lastOff u32 | longLen u32 | cnt u8 | cap u8
     // S2 modes: per-warp output windows in the candidate bitmaps (dead after the walk); a thread's piece is < 400 bytes
     static constexpr uint32_t SM_STG = SM_BM;
     static constexpr uint32_t STG_S2 = ((BM_BYTES * (C::LONG ? 2u : 1u)) / (C::NT / 32)) & ~15u;
-    static constexpr uint32_t SM_SH = SM_ARR + C::NT * 14;
+    static constexpr uint32_t SM_SH = BEST ? SM_BML + BM_BYTES : SM_ARR + C::NT * 14;
     static constexpr uint32_t SMEM_BYTES = SM_SH + ((sizeof(ParseShared) + 2 * 80 * 4 + 15) / 16) * 16;
-    // per-CTA global scratch: candidate distances (u16 per position) + spilled match records [k][thread]
-    static constexpr uint32_t DIST_BYTES = C::BLOCK * 2;
+    // per-CTA global scratch: candidate distances (u16 per position; four per position for S2 best) + spilled match
+    // records [k][thread]
+    static constexpr uint32_t DIST_BYTES = C::BLOCK * (LV == LZ_S2BEST ? 8 : 2);
     static constexpr uint32_t SCRATCH_BYTES = DIST_BYTES + (LZ_MAXREC - C::KREC) * C::NT * 4;
 };
 static_assert(2 * (LzLayout<1>::SMEM_BYTES + 1024) <= 228 * 1024, "two level-1 parse CTAs must fit one SM");
 static_assert(LzLayout<2>::SMEM_BYTES <= 227 * 1024 && LzLayout<5>::SMEM_BYTES <= 227 * 1024, "the level-2 / level-3 parse CTA must fit one SM");
 static_assert(2 * (LzLayout<3>::SMEM_BYTES + 1024) <= 228 * 1024 && 2 * (LzLayout<4>::SMEM_BYTES + 1024) <= 228 * 1024, "two S2 parse CTAs must fit one SM");
+static_assert(LzLayout<6>::SMEM_BYTES <= 227 * 1024, "the S2 best parse CTA must fit one SM");
+static_assert(LzLayout<6>::SM_ARR + LzCfg<6>::NT * 14 <= LzLayout<6>::A_BYTES, "best: records and arrays must lie in the dead tables");
 
 // hashes: two 32-bit multiply-adds (the reference's hashLen is a 64-bit multiply, zstd/hash.go:27-33; table contents
 // are an implementation detail, only verified matches reach the output)
@@ -299,6 +324,136 @@ B2C_DEV void lz_dense_tile(uint32_t *TS, uint32_t *TL, uint32_t *bm, uint32_t *b
     }
 }
 
+// The S2 best form of lz_dense_tile (one position per thread and tile, both tables): the position keeps all four
+// candidates it was offered -- near and far of the long table, near and far of the short table -- as u16 distances
+// (0 = none) in cd4[4 * position ..], and the bitmap marks the positions with at least one.  (One position per thread
+// makes a tile 512 positions, so "near" lies at most 512 bytes back: what a copy tag with a short offset needs.)
+template <bool GUARD>
+B2C_DEV void lz_dense_tile_best(uint32_t *TS, uint32_t *TL, uint32_t *bm, uint16_t *cd4, uint32_t g, uint32_t npos,
+                                const uint32_t (&wv)[3], unsigned lane) {
+    using C = LzCfg<LZ_S2BEST>;
+    static_assert(C::PPT == 1, "one position per thread and tile");
+    constexpr uint32_t BAD = 0x80000000u | LZ_TAGMASK;
+    constexpr uint32_t KX = LZ_KEYX<C::NT>;
+    const uint32_t p0 = g, sh = (g & 3u) * 8;
+    const uint32_t lo = __funnelshift_r(wv[0], wv[1], sh), hi = __funnelshift_r(wv[1], wv[2], sh);
+    const uint32_t hs = lz_hash_short<C::SMLS>(lo, hi), hl = lz_hash_long<C::LMLS>(lo, hi);
+    const uint32_t is = hs >> (32 - C::TBITS), il = hl >> (32 - LZ_BEST_LBITS);
+    const uint32_t es = (p0 << LZ_TAGBITS) | (hs & LZ_TAGMASK), el = (p0 << LZ_TAGBITS) | (hl & LZ_TAGMASK);
+    const uint32_t fs = TS[is] ^ KX, fl = TL[il] ^ KX;
+    __syncthreads();
+    const bool live = !GUARD || p0 < npos;
+    if (live) { atomicMax(&TS[is], es ^ KX); atomicMax(&TL[il], el ^ KX); }
+    __syncthreads();
+    uint32_t d[4] = {0, 0, 0, 0};
+    if (live) {
+        const uint32_t tln = el - (TL[il] ^ KX), tlf = el - fl;
+        const uint32_t tsn = es - (TS[is] ^ KX), tsf = es - fs;
+        if ((tln & BAD) == 0 && tln != 0) d[0] = tln >> LZ_TAGBITS;
+        if ((tlf & BAD) == 0 && tlf != 0) d[1] = tlf >> LZ_TAGBITS;
+        if ((tsn & BAD) == 0 && tsn != 0) d[2] = tsn >> LZ_TAGBITS;
+        if ((tsf & BAD) == 0 && tsf != 0) d[3] = tsf >> LZ_TAGBITS;
+        if (d[1] == d[0]) d[1] = 0;                       // (one position offered twice is scored once)
+        if (d[2] == d[0] || d[2] == d[1]) d[2] = 0;
+        if (d[3] == d[0] || d[3] == d[1] || d[3] == d[2]) d[3] = 0;
+    }
+    const uint32_t w0 = d[0] | (d[1] << 16), w1 = d[2] | (d[3] << 16);
+    reinterpret_cast<uint2 *>(cd4)[p0] = make_uint2(w0, w1);
+    const unsigned word = __ballot_sync(FULLMASK, (w0 | w1) != 0);
+    if (lane == 0) bm[g >> 5] = word;
+}
+
+// emitCopyNoRepeatSize (s2/encode_best.go:756-773): the Snappy best parse scores with this estimate, which for long
+// copies is above what the emitter writes
+B2C_DEV uint32_t snappy_copy_size_est(uint32_t off, uint32_t len) {
+    if (len > 64) return 3 + 3 * (len / 60);
+    return (len >= 12 || off >= 2048) ? 3u : 2u;
+}
+
+// Forward match length of positions p and cand (cand < p) in the staged chunk, at most lim - p
+B2C_DEV uint32_t lz_fwd_len(const uint32_t *srcw, uint32_t p, uint32_t cand, uint32_t lim) {
+    uint32_t len = 0, ia = p >> 2, ib = cand >> 2;
+    const uint32_t sha = (p & 3) * 8, shb = (cand & 3) * 8;
+    uint32_t wa0 = srcw[ia], wb0 = srcw[ib];
+    while (p + len < lim) {
+        const uint32_t wa1 = srcw[++ia], wb1 = srcw[++ib];
+        const uint32_t x = __funnelshift_r(wa0, wa1, sha) ^ __funnelshift_r(wb0, wb1, shb);
+        if (x) { len += (uint32_t)(__ffs((int)x) - 1) >> 3; break; }
+        len += 4; wa0 = wa1; wb0 = wb1;
+    }
+    return len < lim - p ? len : lim - p;
+}
+
+// The S2 best walk of one thread over [b, pend): encodeBlockBest's search (s2/encode_best.go:78-368) on the dense
+// pass's candidates.  At every position s: the four candidates of s and the repeat at s+1; once one is usable, the four
+// of s+1, the repeat and the four of s+2, and the match-end probe (the long-table candidates at the best match's end,
+// moved back by its length).  Each is scored as the reference does (length - s, +1 without literals, minus the size of
+// its copy or repeat tag; a candidate without saving is dropped, ties keep the earlier) and the best is extended
+// backwards (not a repeat) and recorded.  The repeat offset is the thread's previous match's (none at the range start).
+// Every candidate starts inside the range, so the records keep the range-relative form of lz_rec.
+template <int MODE>
+B2C_DEV void lz_walk_best(const uint8_t *src, const uint32_t *bm, const uint16_t *cd4, uint32_t b, uint32_t pend, uint32_t npos,
+                          uint32_t n, uint32_t tid, uint32_t *recS, uint32_t *recG, uint32_t &cnt, uint32_t &lastE, bool &capped) {
+    using C = LzCfg<LZ_S2BEST>;
+    constexpr bool SNAPPY = (MODE == LZ_MODE_SNAPPY);
+    const uint32_t *srcw = reinterpret_cast<const uint32_t *>(src);
+    uint32_t p = b, nextEmit = b, rep = 0;
+    while (p < pend) {
+        uint32_t bs = 0, bd = 0, bl = 0;        // best: start, distance, length (bl = 0: none)
+        int bkey = 0;                           // score - s, the quantity bestOf compares
+        bool brep = false, bcap = false;
+        auto eval = [&](uint32_t s, uint32_t d, bool isRep) {
+            if (d == 0 || d > s || s >= pend) return;
+            if (bl != 0 && bd == d) return;                                    // same offset: not retested
+            const uint32_t lim = (s + LZ_EXT_CAP < n) ? s + LZ_EXT_CAP : n;
+            const uint32_t len = lz_fwd_len(srcw, s, s - d, lim);
+            if (len < 4) return;
+            const uint32_t tag = SNAPPY ? snappy_copy_size_est(d, len) : (isRep ? s2_repeat_size(d, len) : s2_copy_size(d, len));
+            const int val = (int)len + (s == nextEmit ? 1 : 0) - (int)tag;       // score + s
+            if (val <= 0) return;                                              // no saving
+            const int key = val - 2 * (int)s;
+            if (bl != 0 && bkey >= key) return;
+            bs = s; bd = d; bl = len; bkey = key; brep = isRep; bcap = (len == lim - s) && lim < n;
+        };
+        auto evalPos = [&](uint32_t s) {
+            if (s >= pend || !((bm[s >> 5] >> (s & 31)) & 1)) return;
+            const uint2 c = reinterpret_cast<const uint2 *>(cd4)[s];
+            eval(s, c.x & 0xffffu, false); eval(s, c.x >> 16, false);
+            eval(s, c.y & 0xffffu, false); eval(s, c.y >> 16, false);
+        };
+        evalPos(p);
+        if (rep) eval(p + 1, rep, !SNAPPY);
+        if (bl != 0) {
+            evalPos(p + 1);
+            if (rep) eval(p + 2, rep, !SNAPPY);
+            evalPos(p + 2);
+            // match end (skipBeginning 2 / skipEnd 1 for S2, the exact end for Snappy)
+            constexpr uint32_t SKB = SNAPPY ? 0 : 2, SKE = SNAPPY ? 0 : 1;
+            const uint32_t sAt = bs + bl - SKE, sBack = bs + SKB - SKE, backL = bl - SKB;
+            if (sAt < npos && ((bm[sAt >> 5] >> (sAt & 31)) & 1)) {
+                const uint32_t c = reinterpret_cast<const uint32_t *>(cd4)[2 * sAt];         // the long table's pair
+#pragma unroll
+                for (int k = 0; k < 2; k++) {
+                    const uint32_t dl = k ? c >> 16 : c & 0xffffu;
+                    if (dl && dl <= sAt && sAt - dl > backL) eval(sBack, sBack - (sAt - dl - backL), false);
+                }
+            }
+        }
+        if (bl == 0) { p++; continue; }
+        uint32_t s = bs, len = bl;
+        if (!brep)
+            while (s > nextEmit && s > bd && src[s - 1] == src[s - bd - 1]) { s--; len++; }
+        const uint32_t rec = lz_rec(s - b, len, bd);
+        if (cnt < C::KREC) recS[cnt * C::NT + tid] = rec; else recG[(cnt - C::KREC) * C::NT + tid] = rec;
+        cnt++;
+        capped = bcap;
+        rep = bd;
+        p = s + len;
+        nextEmit = p;
+    }
+    if (cnt) lastE = nextEmit;
+}
+
 // One warp writes staging bytes [ph, ph + fill) to gd[0, fill): the staging offset has the destination's 16-byte phase, so
 // the middle leaves as 16-byte vectors and only the ragged ends use byte stores.
 B2C_DEV void lz_warp_flush(const uint8_t *stg, uint32_t ph, uint32_t fill, uint8_t *gd, unsigned lane) {
@@ -354,7 +509,7 @@ B2C_DEV void lz_parse_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chun
     }
     B2C_PHASE(0);
     // ---------------------------------------------------------------- P0: empty tables
-    for (uint32_t i = tid; i < L::NTAB * TSIZE; i += NT) TS[i] = LZ_EMPTY<NT * C::PPT>;
+    for (uint32_t i = tid; i < L::TAB_BYTES / 4; i += NT) TS[i] = LZ_EMPTY<NT * C::PPT>;
     if (tid < 16) {
         uint32_t sel = 0, k = 0;
         for (uint32_t bb = 0; bb < 4; bb++)
@@ -403,8 +558,13 @@ B2C_DEV void lz_parse_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chun
                     for (int q = 0; q < NWRD; q++) LZ_WORD(nwv[q], LZ_WI(g + NT) + q);
                 }
             }
+            if constexpr (LV == LZ_S2BEST) {
+                if (PPT * (k + 1) * NT <= npos) lz_dense_tile_best<false>(TS, TL, bm, cd, g, npos, wv, lane);
+                else lz_dense_tile_best<true>(TS, TL, bm, cd, g, npos, wv, lane);
+            } else {
             if (PPT * (k + 1) * NT <= npos) lz_dense_tile<LV, false>(TS, TL, bm, bml, cd, g, npos, wv, lane);
             else lz_dense_tile<LV, true>(TS, TL, bm, bml, cd, g, npos, wv, lane);
+            }
 #pragma unroll
             for (int q = 0; q < NWRD; q++) wv[q] = nwv[q];
         }
@@ -464,7 +624,10 @@ B2C_DEV void lz_parse_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chun
     const uint32_t e = (b + LZ_RANGE < n) ? b + LZ_RANGE : n;
     uint32_t cnt = 0, lastE = 0;
     bool capped = false;
-    {
+    if constexpr (LV == LZ_S2BEST) {
+        const uint32_t pend = (tid < nlanes) ? (e < npos ? e : npos) : 0u;
+        lz_walk_best<MODE>(src, bm, cd, b, pend, npos, n, tid, recS, recG, cnt, lastE, capped);
+    } else {
         const uint32_t pend = (tid < nlanes) ? (e < npos ? e : npos) : 0u;
         uint32_t p = b > hist ? b : hist, nextEmit = p;            // (history is never walked, nor extended into backwards)
         while (p < pend) {
@@ -604,7 +767,9 @@ B2C_DEV void lz_parse_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chun
         uint8_t *gdst = P.dst_base + (uint64_t)chunk * P.dst_stride;
         // encodeBlock's "not compressible" rule (s2/encode_all.go:88: dstLimit), blocks below minNonLiteralBlockSize
         // (s2/encode.go:375) and the empty input are stored as one literal
-        const bool store = (n < 32) || (nseq == 0) || (body > n - (n >> 5) - 5);
+        // (S2 best: encodeBlockBest's dstLimit = n - 5, s2/encode_best.go:53, on everything but the last literal header)
+        const bool store = (LV == LZ_S2BEST) ? (n < 32 || bodyNoTail + tl > n - 5)
+                                             : ((n < 32) || (nseq == 0) || (body > n - (n >> 5) - 5));
         const uint32_t total = hdrLen + (store ? s2_lit_hdr_size(n) + n : body);
         if (total > P.dst_cap) {
             if (tid == 0) P.out_sizes[chunk] = -4;
@@ -1021,6 +1186,8 @@ B2C_LZ_KERNEL(b2c_lz_s2_fast_kernel, 3, LZ_MODE_S2)
 B2C_LZ_KERNEL(b2c_lz_snappy_fast_kernel, 3, LZ_MODE_SNAPPY)
 B2C_LZ_KERNEL(b2c_lz_s2_better_kernel, 4, LZ_MODE_S2)
 B2C_LZ_KERNEL(b2c_lz_snappy_better_kernel, 4, LZ_MODE_SNAPPY)
+B2C_LZ_KERNEL(b2c_lz_s2_best_kernel, LZ_S2BEST, LZ_MODE_S2)
+B2C_LZ_KERNEL(b2c_lz_snappy_best_kernel, LZ_S2BEST, LZ_MODE_SNAPPY)
 #undef B2C_LZ_KERNEL
 extern "C" __global__ void __launch_bounds__(HIST_NT) b2c_zstd_hist_kernel(ZstdEncParams P) {
     extern __shared__ __align__(1024) uint8_t smem[];

@@ -22,7 +22,15 @@ BLOCK = 1 << 16
 SLOT = BLOCK + 512
 FAST = 1
 BETTER = 2
+BEST = 3
 FLAG_SNAPPY = 1
+
+
+def _level(better=False, best=False):
+    """The block encoder class: FAST, BETTER (s2.EncodeBetter's) or BEST (s2.EncodeBest's); the last two exclude each other."""
+    if better and best:
+        raise ValueError("s2: better and best exclude each other")
+    return BEST if best else (BETTER if better else FAST)
 
 
 class ErrCorrupt(B2CError):
@@ -116,16 +124,17 @@ class Codec:
         return int(lib.b2c_launch_count(self._ctx))
 
     # ---- device-resident batches --------------------------------------------------------------
-    def encode_device(self, src, sizes=None, block=BLOCK, snappy=False, dst=None, out_sizes=None, better=False):
+    def encode_device(self, src, sizes=None, block=BLOCK, snappy=False, dst=None, out_sizes=None, better=False, best=False):
         """src: uint8 CUDA tensor, block i at i*block.  Returns (dst [n, SLOT], out_sizes int64).  Async."""
         assert src.is_cuda and src.dtype == torch.uint8
+        level = _level(better, best)
         n = src.numel() // block if sizes is None else sizes.numel()
         if dst is None:
             dst = torch.empty((n, SLOT), dtype=torch.uint8, device=src.device)
         if out_sizes is None:
             out_sizes = torch.empty((n,), dtype=torch.int64, device=src.device)
         stream = torch.cuda.current_stream(src.device).cuda_stream
-        check(lib.b2c_s2_encode_device(self._ctx, BETTER if better else FAST, FLAG_SNAPPY if snappy else 0, src.data_ptr(), block,
+        check(lib.b2c_s2_encode_device(self._ctx, level, FLAG_SNAPPY if snappy else 0, src.data_ptr(), block,
                                        None if sizes is None else sizes.data_ptr(), block, dst.data_ptr(), SLOT,
                                        out_sizes.data_ptr(), n, ctypes.c_void_p(stream)), self._ctx)
         return dst, out_sizes
@@ -168,10 +177,11 @@ class Codec:
         codes = [int(r) for r in res]
         return [outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes
 
-    def encode_blocks(self, blocks, snappy=False, better=False):
+    def encode_blocks(self, blocks, snappy=False, better=False, best=False):
+        level = _level(better, best)
         if not blocks:
             return []
-        outs, codes = self._host(lib.b2c_s2_encode_chunks, blocks, [MaxEncodedLen(len(b)) + 16 for b in blocks], BETTER if better else FAST,
+        outs, codes = self._host(lib.b2c_s2_encode_chunks, blocks, [MaxEncodedLen(len(b)) + 16 for b in blocks], level,
                                  FLAG_SNAPPY if snappy else 0)
         for c in codes:
             if c == -3:
@@ -185,13 +195,13 @@ class Codec:
             return [], []
         return self._host(lib.b2c_s2_decode_chunks, blocks, caps)
 
-    def _encode_any(self, src, snappy=False, better=False):
+    def _encode_any(self, src, snappy=False, better=False, best=False):
         """One block for an input of any size: pieces of 64 KiB are encoded as one device batch and joined with ConcatBlocks
         (every piece's copies stay inside the piece, so the joined bodies are one valid block)."""
         if len(src) <= BLOCK:
-            return self.encode_blocks([src], snappy=snappy, better=better)[0]
+            return self.encode_blocks([src], snappy=snappy, better=better, best=best)[0]
         src = bytes(src)
-        parts = self.encode_blocks([src[o:o + BLOCK] for o in range(0, len(src), BLOCK)], snappy=snappy, better=better)
+        parts = self.encode_blocks([src[o:o + BLOCK] for o in range(0, len(src), BLOCK)], snappy=snappy, better=better, best=best)
         return ConcatBlocks(parts)
 
     def Encode(self, src):
@@ -209,6 +219,14 @@ class Codec:
     def EncodeSnappy(self, src):
         """s2.EncodeSnappy(nil, src) (s2/encode.go:204): output any Snappy decoder accepts."""
         return self._encode_any(src, snappy=True)
+
+    def EncodeBest(self, src):
+        """s2.EncodeBest(nil, src) (s2/encode.go:161): the cost-scored match finder, for data written once and read often."""
+        return self._encode_any(src, best=True)
+
+    def EncodeSnappyBest(self, src):
+        """s2.EncodeSnappyBest(nil, src) (s2/encode.go:292)."""
+        return self._encode_any(src, snappy=True, best=True)
 
     def Decode(self, src, max_len=None):
         """s2.Decode(nil, src) (s2/decode.go:58); max_len defaults to the block's own declared length."""
@@ -265,14 +283,15 @@ class Codec:
         return dst, out_sizes, decoded
 
     # ---- streams: the framing format (s2.Writer.EncodeBuffer / s2.Reader, s2/writer.go:357-470, s2/reader.go:249-420) ----
-    def EncodeStream(self, src, better=False, snappy=False, block_size=BLOCK, index=False):
+    def EncodeStream(self, src, better=False, snappy=False, block_size=BLOCK, index=False, best=False):
         """Writer.EncodeBuffer(src) + Close(): a complete S2 (or Snappy) stream -- identifier, one checksummed chunk per
         block.  block_size <= 64 KiB (WriterBlockSize)."""
+        level = _level(better, best)
         buf = np.frombuffer(src, dtype=np.uint8) if len(src) else np.zeros(0, dtype=np.uint8)
         cap = int(lib.b2c_s2_stream_bound(len(src), block_size)) + 16
         out = np.empty(cap, dtype=np.uint8)
         n = ctypes.c_size_t(0)
-        rc = lib.b2c_s2_encode_stream(self._ctx, BETTER if better else FAST, FLAG_SNAPPY if snappy else 0, buf.ctypes.data, len(src),
+        rc = lib.b2c_s2_encode_stream(self._ctx, level, FLAG_SNAPPY if snappy else 0, buf.ctypes.data, len(src),
                                       block_size, out.ctypes.data, cap, ctypes.byref(n))
         check(rc, self._ctx)
         stream = out[: n.value].tobytes()
@@ -286,16 +305,17 @@ class Codec:
         appended to the stream."""
         return s2_index.read_range(stream, start, length, self.DecodeStream, index)
 
-    def encode_stream_device(self, src, better=False, snappy=False, block_size=BLOCK, dst=None):
+    def encode_stream_device(self, src, better=False, snappy=False, block_size=BLOCK, dst=None, best=False):
         """src: uint8 CUDA tensor.  Returns (dst uint8 CUDA tensor, total uint64 CUDA tensor [1], err int32 CUDA tensor [1]).  Async."""
         assert src.is_cuda and src.dtype == torch.uint8
+        level = _level(better, best)
         n = src.numel()
         if dst is None:
             dst = torch.empty(int(lib.b2c_s2_stream_bound(n, block_size)) + 16, dtype=torch.uint8, device=src.device)
         total = torch.zeros(1, dtype=torch.uint64, device=src.device)
         err = torch.zeros(1, dtype=torch.int32, device=src.device)
         stream = torch.cuda.current_stream(src.device).cuda_stream
-        rc = lib.b2c_s2_encode_stream_device(self._ctx, BETTER if better else FAST, FLAG_SNAPPY if snappy else 0, src.data_ptr(), n,
+        rc = lib.b2c_s2_encode_stream_device(self._ctx, level, FLAG_SNAPPY if snappy else 0, src.data_ptr(), n,
                                              block_size, dst.data_ptr(), dst.numel(), total.data_ptr(), err.data_ptr(),
                                              ctypes.c_void_p(stream))
         check(rc, self._ctx)
@@ -370,15 +390,17 @@ class Writer:
     the device stream encoder: input is gathered and leaves in batches of `batch_bytes` (a multiple of the block size) through
     ONE EncodeStream call each -- all blocks of the batch in parallel -- with the stream identifier kept on the first batch
     only.  add_index = WriterAddIndex, padding = WriterPadding (the padding chunk comes before the index so that the index
-    stays at the end), better / snappy / block_size = WriterBetterCompression / WriterSnappyCompat / WriterBlockSize."""
+    stays at the end), better / best / snappy / block_size = WriterBetterCompression / WriterBestCompression /
+    WriterSnappyCompat / WriterBlockSize."""
 
     def __init__(self, w, codec=None, device=0, block_size=BLOCK, better=False, snappy=False, add_index=False, padding=0,
-                 batch_bytes=8 << 20, rand=None, flush_on_write=False):
+                 batch_bytes=8 << 20, rand=None, flush_on_write=False, best=False):
+        _level(better, best)
         if not 4096 <= block_size <= BLOCK:
             raise ErrUnsupported("s2: block size on the device path: 4 KiB .. 64 KiB")
         self._codec = codec if codec is not None else Codec(device=device)
         self._own = codec is None
-        self._bs, self._better, self._snappy = block_size, better, snappy
+        self._bs, self._better, self._snappy, self._best = block_size, better, snappy, best
         self._add_index, self._pad, self._rand = add_index, padding, rand
         self._flush_on_write = flush_on_write               # WriterFlushOnWrite: nothing stays buffered after Write
         self._batch = max(block_size, batch_bytes // block_size * block_size)
@@ -399,7 +421,11 @@ class Writer:
         self.written += len(b)
 
     def _emit(self, data):
-        piece = self._codec.EncodeStream(bytes(data), better=self._better, snappy=self._snappy, block_size=self._bs)
+        # A Writer takes any codec with EncodeStream(data, better=, snappy=, block_size=); `best` is passed only when
+        # that level is asked for, so a codec that knows the first two levels (such as a host model of the format)
+        # still serves them.
+        extra = {"best": True} if self._best else {}
+        piece = self._codec.EncodeStream(bytes(data), better=self._better, snappy=self._snappy, block_size=self._bs, **extra)
         body = piece[10:]
         if not self._wrote_header:
             self._out(piece[:10])

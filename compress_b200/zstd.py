@@ -878,10 +878,12 @@ class Queue:
     def DecodeAll(self, src, max_size=1 << 20):
         return self._call(lib.b2c_queue_zstd_decode, (), src, max_size)
 
-    def S2Encode(self, src, snappy=False):
-        """The WriterCustomEncoder contract on one block: the encoded block (this mirror keeps the uvarint length)."""
+    def S2Encode(self, src, snappy=False, better=False, best=False):
+        """The WriterCustomEncoder contract on one block: the encoded block (this mirror keeps the uvarint length).
+        better / best: s2.EncodeBetter's / s2.EncodeBest's class."""
+        from .s2 import _level
         cap = int(lib.b2c_s2_bound(len(src)))
-        return self._call(lib.b2c_queue_s2_encode, (1, 1 if snappy else 0), src, cap)
+        return self._call(lib.b2c_queue_s2_encode, (_level(better, best), 1 if snappy else 0), src, cap)
 
     def S2Decode(self, src, max_size=1 << 20):
         return self._call(lib.b2c_queue_s2_decode, (), src, max_size)

@@ -53,8 +53,12 @@ enum {
 /* S2 block encoder: level and flags.  B2C_S2_FAST = s2.Encode's match finder class (s2/encode.go:29, encodeBlockGo),
  * B2C_S2_BETTER = s2.EncodeBetter's (s2/encode.go:117, encodeBlockBetterGo64K in s2/encode_better.go:485: long 7-byte +
  * short 4-byte table, long preferred, lazy step).  B2C_S2_SNAPPY selects Snappy-compatible output (s2.EncodeSnappy /
- * EncodeSnappyBetter, s2/encode.go:204,248: no repeat tags, copies <= 64). */
-enum { B2C_S2_FAST = 1, B2C_S2_BETTER = 2 };
+ * EncodeSnappyBetter, s2/encode.go:204,248: no repeat tags, copies <= 64).  B2C_S2_BEST = s2.EncodeBest's class
+ * (s2/encode.go:161, encodeBlockBest in s2/encode_best.go:22: long 8-byte + short 4-byte table, cost-scored choice among
+ * several candidates per position; EncodeSnappyBest with B2C_S2_SNAPPY).  A best block is stored as one literal only
+ * when its tags would not save 5 bytes (the reference's dstLimit = n - 5), so it can be tags where the other levels
+ * store; the stream calls then write a compressed chunk, as s2.Writer does. */
+enum { B2C_S2_FAST = 1, B2C_S2_BETTER = 2, B2C_S2_BEST = 3 };
 enum { B2C_S2_SNAPPY = 1 };
 
 /* huff0: number of streams (huff0.Compress4X / Compress1X, huff0/compress.go:27,14) */
