@@ -523,11 +523,11 @@ B2C_DEV uint32_t huf_enc_sizes(HufWork *hw, uint32_t *pk, const uint8_t *lit, ui
 #undef HSYNC
     return totalBytes;
 }
-// stageBase: 4-byte aligned, zero-initialised words; payload starts at byte offset byteOff.
-// pk: the table huf_enc_sizes filled (a barrier lies between the two calls).
-B2C_DEV void huf_enc_pack(HufWork *hw, const uint32_t *pk, const uint8_t *lit, int four, uint8_t *stageBase,
-                          uint32_t byteOff, unsigned tid, unsigned nthreads, int bar_id, const HufEncState *st) {
-#define HSYNC() do { group_sync(bar_id, (int)nthreads); } while (0)
+// The two halves of huf_enc_pack, for callers that order them against their own stores:
+//   huf_enc_pack_bits   : the streams, word-granular (plain stores and atomicOr into the zeroed staging words)
+//   huf_enc_pack_header : the table description and the jump table, byte stores; a barrier must separate the two.
+B2C_DEV void huf_enc_pack_bits(const uint32_t *pk, const uint8_t *lit, uint8_t *stageBase, uint32_t byteOff,
+                               const HufEncState *st) {
     const HufSeg &sg = st->sg;
     {
         BitRun br;
@@ -554,8 +554,9 @@ B2C_DEV void huf_enc_pack(HufWork *hw, const uint32_t *pk, const uint8_t *lit, i
         if (last) br.add(1u, 1);
         br.finish();
     }
-    HSYNC();
-    // header bytes (byte stores, ordered after the word-granular atomics above)
+}
+B2C_DEV void huf_enc_pack_header(const HufWork *hw, int four, uint8_t *stageBase, uint32_t byteOff, unsigned tid,
+                                 unsigned nthreads) {
     uint8_t *stage = stageBase + byteOff;
     for (unsigned i = tid; i < hw->tableDescLen; i += nthreads) stage[i] = hw->tableDesc[i];
     if (four && tid < 3) {
@@ -563,8 +564,16 @@ B2C_DEV void huf_enc_pack(HufWork *hw, const uint32_t *pk, const uint8_t *lit, i
         stage[hw->tableDescLen + tid * 2] = (uint8_t)L;
         stage[hw->tableDescLen + tid * 2 + 1] = (uint8_t)(L >> 8);
     }
-    HSYNC();
-#undef HSYNC
+}
+// stageBase: 4-byte aligned, zero-initialised words; payload starts at byte offset byteOff.
+// pk: the table huf_enc_sizes filled (a barrier lies between the two calls).
+B2C_DEV void huf_enc_pack(HufWork *hw, const uint32_t *pk, const uint8_t *lit, int four, uint8_t *stageBase,
+                          uint32_t byteOff, unsigned tid, unsigned nthreads, int bar_id, const HufEncState *st) {
+    huf_enc_pack_bits(pk, lit, stageBase, byteOff, st);
+    group_sync(bar_id, (int)nthreads);
+    // header bytes (byte stores, ordered after the word-granular atomics above)
+    huf_enc_pack_header(hw, four, stageBase, byteOff, tid, nthreads);
+    group_sync(bar_id, (int)nthreads);
 }
 
 }  // namespace b2c

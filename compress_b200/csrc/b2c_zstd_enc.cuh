@@ -33,20 +33,14 @@ constexpr uint32_t ENC_MAX_CHUNK = 1u << 16;   // block size of zstd level 1 and
 #ifndef PACK_THREADS
 #define PACK_THREADS 512
 #endif
-#ifndef PACK_SEQ_UNROLL
-#define PACK_SEQ_UNROLL 1
-#endif
-#ifndef PACK_SEQ_COMBINE
-#define PACK_SEQ_COMBINE 1   // 1: state bits of the three chains in one append, LL+ML extra bits in one
-#endif
 #ifndef PACK_BITS_LUT
 #define PACK_BITS_LUT 1      // extra-bit counts from a 2 x 64 byte shared-memory table instead of compare chains
 #endif
 #ifndef PACK_MIN_CTAS
 #define PACK_MIN_CTAS 2   // two CTAs per SM: caps the kernel at 64 registers per thread
 #endif
-constexpr int PACK_UNROLL = PACK_SEQ_UNROLL;   // unroll factor of the two per-sequence loops
 constexpr int PACK_NT = PACK_THREADS;     // K4 threads per CTA (a multiple of 128: four Huffman streams)
+static_assert(PACK_NT % 128 == 0 && PACK_NT >= 384, "K4 loads the Huffman table description with one thread per byte");
 
 enum { ENC_FLAG_CRC = 1, ENC_FLAG_FRAME = 2 };
 
@@ -106,7 +100,7 @@ struct ZstdEncParams {
     uint32_t *dbg_seqs;           // [nchunks][dbg_seq_cap][3]
     uint8_t *dbg_lits;            // [nchunks][65536]
     uint32_t dbg_seq_cap;
-    unsigned long long *dbg_cycles;  // optional [nchunks][16][32] per-warp stamps inside K1 (clock64)
+    unsigned long long *dbg_cycles;  // optional [nchunks][16][32] per-warp stamps inside K1 and K4 (clock64)
 };
 
 #ifdef B2C_EMU
@@ -118,6 +112,17 @@ struct ZstdEncParams {
     do {                                                                                               \
         if (P.dbg_cycles && (threadIdx.x & 31) == 0)                                                   \
             P.dbg_cycles[((uint64_t)chunk * 16 + (k)) * 32 + (threadIdx.x >> 5)] = (unsigned long long)clock64(); \
+    } while (0)
+#endif
+// The same stamps in K4 (tools/pack_phase_times.py): its warps take columns 16..31 of the chunk's rows, beside the
+// parse's 16 warps, so one timed run records both kernels.  Not every stamp follows a barrier here.
+#ifdef B2C_EMU
+#define B2C_PACK_PHASE(k) do { } while (0)
+#else
+#define B2C_PACK_PHASE(k)                                                                              \
+    do {                                                                                               \
+        if (P.dbg_cycles && (threadIdx.x & 31) == 0 && (threadIdx.x >> 5) < 16)                        \
+            P.dbg_cycles[((uint64_t)chunk * 16 + (k)) * 32 + 16 + (threadIdx.x >> 5)] = (unsigned long long)clock64(); \
     } while (0)
 #endif
 
@@ -156,6 +161,13 @@ static inline uint64_t wk_pool_stride(uint32_t blockmax) {
     const uint64_t ms = wk_maxseq(blockmax), lenb = blockmax > 65536 ? 4 : 2;
     return (((uint64_t)blockmax + 64 + 15) & ~15ull) + 4 * ms + 2 * lenb * ms + 3 * ms + 6 * ms;
 }
+// The same layout for a block size known at compile time (K4, whose template BLOCK is the launch's blockmax): every
+// array sits at a constant offset from the slab.
+template <uint32_t BLOCK> struct WkLayout {
+    static constexpr uint32_t MAXSEQ = BLOCK / 4 + 64, LENB = BLOCK > 65536 ? 4u : 2u;
+    static constexpr uint32_t OF = (BLOCK + 64 + 15) & ~15u, LL = OF + 4 * MAXSEQ, ML = LL + LENB * MAXSEQ;
+    static constexpr uint32_t CODES = ML + LENB * MAXSEQ, STB = CODES + 3 * MAXSEQ;
+};
 // litLen / matchLen-3 of sequence i (u16 arrays for blocks <= 64 KiB, u32 above)
 struct WkLens {
     uint8_t *ll, *ml;
@@ -435,7 +447,8 @@ struct PackShared {
                               //   hw.count[256] = Huffman codes as (code | nbits << 16)               (PACK_PK)
                               //   hw.nsym[0..127] = extra-bit counts per LL / ML code, seqenc.go:61-97  (PACK_LLB / PACK_MLB)
     uint32_t scan[40];
-    uint32_t litMode, lhSize, litPayload, pos;
+    uint32_t litMode, lhSize, litPayload, seqOff, total, blockBytes, nc0, nc1;   // the byte phase's layout
+    uint64_t mbar;            // completion of the literals' bulk copy
 };
 #if PACK_BITS_LUT
 #define PACK_LLB(c) ((uint32_t)ps->hw.nsym[(c) & 63])
@@ -485,15 +498,76 @@ B2C_DEV uint32_t write_frame_header(uint8_t *o8, uint32_t n, bool crc) {
     return o;
 }
 
+// huff0 compress(): out >= wantSize => ErrIncompressible (compress.go:155-158, WantLogLess 4), then blockenc.go:534-544:
+// the literals' mode, 0 raw, 1 RLE, 2 compressed (payload: Huffman bytes, meaningful when the table was built)
+B2C_DEV uint32_t lit_mode(int32_t hufStatus, uint32_t payload, uint32_t nlit) {
+    if (hufStatus != HUF_OK) return (hufStatus == HUF_USE_RLE) ? 1u : 0u;
+    if (payload >= nlit - (nlit >> 4)) return 0;
+    if (payload + 5 > nlit) {
+        // compare with the raw representation
+        const uint32_t inBits = 32 - (uint32_t)__clz((int)nlit);
+        const uint32_t szRaw = inBits < 5 ? 1 : (inBits < 12 ? 2 : 3);
+        const uint32_t compBits = payload ? 32 - (uint32_t)__clz((int)payload) : 0;
+        const uint32_t szComp = (compBits <= 10 && inBits <= 10) ? 3 : ((compBits <= 14 && inBits <= 14) ? 4 : 5);
+        if (payload + szComp >= nlit + szRaw) return 0;
+    }
+    return 2;
+}
+// bytes of the literals section header (blockenc.go:153-238)
+B2C_DEV uint32_t lit_header_bytes(uint32_t mode, uint32_t payload, uint32_t nlit) {
+    if (mode == 2) {
+        const uint32_t inBits = 32 - (uint32_t)__clz((int)nlit);
+        const uint32_t compBits = payload ? 32 - (uint32_t)__clz((int)payload) : 0;
+        return (compBits <= 10 && inBits <= 10) ? 3 : ((compBits <= 14 && inBits <= 14) ? 4 : 5);
+    }
+    const uint32_t inBits = nlit ? 32 - (uint32_t)__clz((int)nlit) : 0;
+    return inBits < 5 ? 1 : (inBits < 12 ? 2 : 3);
+}
+// the literals section header, little-endian in its lhSize low bytes
+B2C_DEV uint64_t lit_header(uint32_t mode, uint32_t lhSize, uint32_t nlit, uint32_t payload, bool four) {
+    if (mode == 2) {
+        const uint64_t comp = payload;
+        if (lhSize == 3) return 2u | ((four ? 1u : 0u) << 2) | ((uint64_t)nlit << 4) | (comp << 14);
+        if (lhSize == 4) return 2u | (2u << 2) | ((uint64_t)nlit << 4) | (comp << 18);
+        return 2u | (3u << 2) | ((uint64_t)nlit << 4) | (comp << 22);
+    }
+    const uint64_t ty = (mode == 1) ? 1u : 0u;
+    if (lhSize == 1) return ty | ((uint64_t)nlit << 3);
+    if (lhSize == 2) return ty | (1u << 2) | ((uint64_t)nlit << 4);
+    return ty | (3u << 2) | ((uint64_t)nlit << 4);
+}
+// element j (a compile-time constant after unrolling) of eight u8 / u16 / u32 values loaded together
+B2C_DEV uint32_t u8_of(uint2 v, int j) { return ((j < 4 ? v.x : v.y) >> (8 * (j & 3))) & 255u; }
+B2C_DEV uint32_t u16_of(uint4 v, int j) {
+    const uint32_t w = j < 2 ? v.x : (j < 4 ? v.y : (j < 6 ? v.z : v.w));
+    return (w >> (16 * (j & 1))) & 0xffffu;
+}
+B2C_DEV uint32_t u32_of(uint4 a, uint4 b, int j) {
+    const uint4 v = j < 4 ? a : b;
+    return (j & 3) == 0 ? v.x : ((j & 3) == 1 ? v.y : ((j & 3) == 2 ? v.z : v.w));
+}
+
+// K4, one CTA per chunk.  Barriers: the sequence scan (2), the Huffman sizes (5, shared with huff0), the end of the
+// word-granular phase and the end of the byte-granular phase.
+//   top      literals into shared memory by one bulk copy (waited for where they are first read); the Huffman table,
+//            the per-chunk scalars and the first sequences' codes and state bits requested together; stage zeroed
+//   seq size thread t owns a contiguous run of 8-aligned groups of sequences (thread 0 the top ones: the bitstream runs
+//            from the last sequence to the first); each group is one 8-byte load per code table and one 16-byte
+//            load per state-bit table, its lengths and offsets are prefetched into L2 for the pack pass; block scan
+//   huf size code-length sums and their scan (huf_enc_sizes); every thread then derives the literal mode and all offsets
+//   words    the Huffman streams and the sequence bitstream, each thread its own bit range of the zeroed stage
+//   bytes    frame / block / literals / sequences headers, NCount bytes, the table description, raw or RLE literals,
+//            the checksum, each field by its own thread
+//   write-back, one coalesced copy (raw / RLE blocks skip the stage)
 template <uint32_t BLOCK>
 B2C_DEV void zstd_pack_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chunk) {
     constexpr uint32_t PACK_STAGE_BYTES = PackCfg<BLOCK>::STAGE_BYTES;
     constexpr uint32_t PACK_LIT_SMEM = PackCfg<BLOCK>::LIT_SMEM;
+    constexpr bool BIG = BLOCK > 65536;   // litLen / matchLen arrays are u32 (P.big)
     const unsigned tid = threadIdx.x;
     uint8_t *stage = smem;
     PackShared *ps = reinterpret_cast<PackShared *>(smem + PackCfg<BLOCK>::SMEM_SH);
     ChunkWork *W = P.work + chunk;
-    const uint8_t *gsrc = chunk_src(P, chunk);
     uint8_t *gdst = P.dst_base + (uint64_t)chunk * P.dst_stride;
     const uint32_t n = W->n;
     const uint32_t lastBit = chunk_last(P, chunk);
@@ -503,136 +577,172 @@ B2C_DEV void zstd_pack_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chu
     if (kind == 3) { if (tid == 0) P.out_sizes[chunk] = -3; return; }
     const uint32_t nseq = W->nseq, nlit = W->nlit;
     const uint32_t fh = frame ? frame_header_bytes(n) : 0;
+    B2C_PACK_PHASE(0);
 
     if (kind == 0) {
-        const uint8_t *lit = wk_lit(P, chunk);
-        if (nlit <= PACK_LIT_SMEM) {
-            uint8_t *ls = smem + PACK_STAGE_BYTES;
-            const uint4 *g4 = reinterpret_cast<const uint4 *>(lit);
-            uint4 *s4 = reinterpret_cast<uint4 *>(ls);
-            for (uint32_t i = tid; i < (nlit + 15) / 16; i += PACK_NT) s4[i] = g4[i];
-            lit = ls;
+        // ------------------------------------------------------------ literals: one bulk copy into shared memory
+        using L = WkLayout<BLOCK>;
+        const uint8_t *slab = wk_slab(P, chunk);
+        const uint8_t *lit = slab;
+        uint8_t *ls = smem + PACK_STAGE_BYTES;
+        const bool litSmem = nlit <= PACK_LIT_SMEM;
+#ifndef B2C_EMU
+        // rounded up to 16 bytes: the slab's literal area has 64 bytes behind the largest block
+        const bool bulk = litSmem && nlit > 0 && (reinterpret_cast<uintptr_t>(lit) & 15) == 0;
+        if (bulk && tid == 0) {
+            mbar_init(&ps->mbar, 1);
+            mbar_fence_init();
+            mbar_expect_tx(&ps->mbar, (nlit + 15) & ~15u);
+            tma_load_1d(ls, lit, (nlit + 15) & ~15u, &ps->mbar);
         }
+#else
+        const bool bulk = false;
+#endif
+        if (litSmem && !bulk) {   // ordered before the first read by the sequence scan's barriers
+            if ((reinterpret_cast<uintptr_t>(lit) & 15) == 0) {
+                const uint4 *g4 = reinterpret_cast<const uint4 *>(lit);
+                for (uint32_t i = tid; i < (nlit + 15) / 16; i += PACK_NT) reinterpret_cast<uint4 *>(ls)[i] = g4[i];
+            } else {
+                for (uint32_t i = tid; i < nlit; i += PACK_NT) ls[i] = lit[i];
+            }
+        }
+        // ------------------------------------------------------------ requests: Huffman table, chunk scalars
         HufWork *hw = &ps->hw;
-        // Huffman table into shared memory
+        uint32_t ctv = 0, ctb = 0, tdb = 0;
+        if (tid < 256) { ctv = W->ctVal[tid]; ctb = W->ctBits[tid]; }
+        if (tid < 320) tdb = W->tableDesc[tid];   // all 320 bytes: no wait for tableDescLen
+        const int32_t hufStatus = (int32_t)W->hufStatus;
+        const uint32_t tableDescLen = W->tableDescLen;
+        const uint32_t nc0 = W->ncountLen[0], nc1 = W->ncountLen[1], ncSum = nc0 + nc1 + W->ncountLen[2];
+        const uint32_t tlLL = W->tbl[TBL_LL].tableLog, tlOF = W->tbl[TBL_OF].tableLog, tlML = W->tbl[TBL_ML].tableLog;
+        // the stage holds the output; zero every word a bit writer may OR into.  A compressed block is smaller than the
+        // chunk (else it is stored raw), so everything it writes lies below fh + 3 + n + 4.
+        {
+            const uint32_t zb = fh + 3 + n + 4 + 8;
+            const uint32_t z16 = (zb < PACK_STAGE_BYTES ? zb + 15 : PACK_STAGE_BYTES) / 16;
+            for (uint32_t i = tid; i < z16; i += PACK_NT) reinterpret_cast<uint4 *>(stage)[i] = make_uint4(0, 0, 0, 0);
+        }
+        B2C_PACK_PHASE(5);
+
+        // ------------------------------------------------------------ sequence bitstream sizes
+        const uint2 *cLL = reinterpret_cast<const uint2 *>(slab + L::CODES + TBL_LL * L::MAXSEQ);
+        const uint2 *cOF = reinterpret_cast<const uint2 *>(slab + L::CODES + TBL_OF * L::MAXSEQ);
+        const uint2 *cML = reinterpret_cast<const uint2 *>(slab + L::CODES + TBL_ML * L::MAXSEQ);
+        const uint4 *stbLL = reinterpret_cast<const uint4 *>(slab + L::STB + 2 * TBL_LL * L::MAXSEQ);
+        const uint4 *stbOF = reinterpret_cast<const uint4 *>(slab + L::STB + 2 * TBL_OF * L::MAXSEQ);
+        const uint4 *stbML = reinterpret_cast<const uint4 *>(slab + L::STB + 2 * TBL_ML * L::MAXSEQ);
+        const uint4 *wll = reinterpret_cast<const uint4 *>(slab + L::LL), *wml = reinterpret_cast<const uint4 *>(slab + L::ML);
+        const uint4 *wof = reinterpret_cast<const uint4 *>(slab + L::OF);
+        // groups of eight sequences [gLo, gHi); entries past nseq are read (the arrays hold maxseq, a multiple of 16)
+        // and ignored, and sequence nseq-1 has no state bits (its states start the chains)
+        const uint32_t ngrp = (nseq + 7) >> 3, gper = (ngrp + PACK_NT - 1) / PACK_NT;
+        const uint32_t gHi = ngrp > tid * gper ? ngrp - tid * gper : 0u, gLo = gHi > gper ? gHi - gper : 0u;
+        uint32_t mybits = 0;
+        for (uint32_t g = gLo; g < gHi; g++) {
+            const uint2 cl8 = B2C_LDG(cLL + g);
+            const uint2 co8 = B2C_LDG(cOF + g);
+            const uint2 cm8 = B2C_LDG(cML + g);
+            const uint4 sl8 = B2C_LDG(stbLL + g);
+            const uint4 so8 = B2C_LDG(stbOF + g);
+            const uint4 sm8 = B2C_LDG(stbML + g);
+            prefetch_l2(wof + 2 * g);
+            prefetch_l2(wll + (BIG ? 2 : 1) * g);
+            prefetch_l2(wml + (BIG ? 2 : 1) * g);
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                const uint32_t idx = 8 * g + j;
+                uint32_t b = seq_ll_bits(u8_of(cl8, j)) + seq_ml_bits(u8_of(cm8, j)) + u8_of(co8, j);
+                if (idx + 1 < nseq) b += (u16_of(sl8, j) >> 12) + (u16_of(so8, j) >> 12) + (u16_of(sm8, j) >> 12);
+                if (idx < nseq) mybits += b;
+            }
+        }
+        if (tid < 256) { hw->ctVal[tid] = (uint16_t)ctv; hw->ctBits[tid] = (uint8_t)ctb; }
+        if (tid < 320) hw->tableDesc[tid] = (uint8_t)tdb;
         if (tid < 64) { ps->hw.nsym[tid] = (uint8_t)seq_ll_bits(tid); ps->hw.nsym[64 + tid] = (uint8_t)seq_ml_bits(tid); }
-        for (uint32_t s = tid; s < 256; s += PACK_NT) { hw->ctVal[s] = W->ctVal[s]; hw->ctBits[s] = W->ctBits[s]; }
-        for (uint32_t i = tid; i < W->tableDescLen; i += PACK_NT) hw->tableDesc[i] = W->tableDesc[i];
-        if (tid == 0) { hw->tableDescLen = W->tableDescLen; hw->status = (int32_t)W->hufStatus; }
-        __syncthreads();
+        if (tid == 0) hw->tableDescLen = tableDescLen;
+        uint32_t totalBits;
+        const uint32_t exBits = group_scan_excl(mybits, ps->scan, 0, PACK_NT, tid, &totalBits);   // also publishes the table
+        B2C_PACK_PHASE(4);
+
         // ------------------------------------------------------------ literals section sizes
+#ifndef B2C_EMU
+        if (bulk) mbar_wait(&ps->mbar, 0);
+#endif
+        if (litSmem) lit = ls;
+        B2C_PACK_PHASE(1);
         const bool four = nlit >= 1024;
         HufEncState hst;
         uint32_t payload = 0;
-        const bool hufOK = hw->status == HUF_OK;
-        if (hufOK) payload = huf_enc_sizes(hw, ps->hw.count, lit, nlit, four ? 1 : 0, tid, PACK_NT, 0, &hst);
-        if (tid == 0) {
-            // huff0 compress(): out >= wantSize => ErrIncompressible (compress.go:155-158, WantLogLess 4)
-            uint32_t mode = 2;
-            if (!hufOK) mode = (hw->status == HUF_USE_RLE) ? 1u : 0u;
-            else {
-                uint32_t wantSize = nlit - (nlit >> 4);
-                if (payload >= wantSize) mode = 0;
-                else if (payload + 5 > nlit) {
-                    // blockenc.go:534-544: compare with the raw representation
-                    uint32_t inBits = 32 - (uint32_t)__clz((int)nlit);
-                    uint32_t szRaw = inBits < 5 ? 1 : (inBits < 12 ? 2 : 3);
-                    uint32_t compBits = payload ? 32 - (uint32_t)__clz((int)payload) : 0;
-                    uint32_t szComp = (compBits <= 10 && inBits <= 10) ? 3 : ((compBits <= 14 && inBits <= 14) ? 4 : 5);
-                    if (payload + szComp >= nlit + szRaw) mode = 0;
-                }
-            }
-            uint32_t lh;
-            if (mode == 2) {
-                uint32_t inBits = 32 - (uint32_t)__clz((int)nlit);
-                uint32_t compBits = payload ? 32 - (uint32_t)__clz((int)payload) : 0;
-                lh = (compBits <= 10 && inBits <= 10) ? 3 : ((compBits <= 14 && inBits <= 14) ? 4 : 5);
-            } else {
-                uint32_t inBits = nlit ? 32 - (uint32_t)__clz((int)nlit) : 0;
-                lh = inBits < 5 ? 1 : (inBits < 12 ? 2 : 3);
-            }
-            ps->litMode = mode; ps->lhSize = lh; ps->litPayload = payload;
-        }
-        __syncthreads();
-        const uint32_t litMode = ps->litMode, lhSize = ps->lhSize;
-        const uint32_t litOff = fh + 3 + lhSize;  // staging offset of the literal payload
-        const uint32_t litBytes = (litMode == 2) ? ps->litPayload : (litMode == 1 ? 1u : nlit);
+        if (hufStatus == HUF_OK) payload = huf_enc_sizes(hw, ps->hw.count, lit, nlit, four ? 1 : 0, tid, PACK_NT, 0, &hst);
+        B2C_PACK_PHASE(2);
+        // every thread derives the layout; the byte phase reads it back from shared memory, so it is not held in
+        // registers across the bit writers
         const uint32_t nsHdr = (nseq < 128) ? 1u : (nseq < 0x7f00 ? 2u : 3u);
-        const uint32_t seqOff = litOff + litBytes;
-        const uint32_t tblOff = seqOff + nsHdr + 1;
-        const uint32_t bsOff = tblOff + W->ncountLen[0] + W->ncountLen[1] + W->ncountLen[2];
-
-        // ------------------------------------------------------------ sequence bitstream sizes
-        const uint8_t *cLL = wk_codes(P, chunk, TBL_LL), *cOF = wk_codes(P, chunk, TBL_OF), *cML = wk_codes(P, chunk, TBL_ML);
-        const uint16_t *stbLL = wk_stb(P, chunk, TBL_LL), *stbOF = wk_stb(P, chunk, TBL_OF), *stbML = wk_stb(P, chunk, TBL_ML);
-        const WkLens wlen = wk_lens(P, chunk);
-        const uint32_t *wof = wk_of(P, chunk);
-        const uint32_t per = (nseq + PACK_NT - 1) / PACK_NT;
-        uint32_t tA = tid * per, tB = tA + per;
-        if (tA > nseq) tA = nseq;
-        if (tB > nseq) tB = nseq;
-        uint32_t mybits = 0;
-#pragma unroll PACK_UNROLL
-        for (uint32_t t = tA; t < tB; t++) {
-            uint32_t idx = nseq - 1 - t;
-            uint32_t cl = B2C_LDG(cLL + idx), co = B2C_LDG(cOF + idx), cm = B2C_LDG(cML + idx);
-            mybits += PACK_LLB(cl) + PACK_MLB(cm) + co;
-            if (t) mybits += (uint32_t)(B2C_LDG(stbLL + idx) >> 12) + (uint32_t)(B2C_LDG(stbOF + idx) >> 12) + (uint32_t)(B2C_LDG(stbML + idx) >> 12);
-        }
-        uint32_t totalBits;
-        uint32_t exBits = group_scan_excl(mybits, ps->scan, 0, PACK_NT, tid, &totalBits);
-        const uint32_t tlLL = W->tbl[TBL_LL].tableLog, tlOF = W->tbl[TBL_OF].tableLog, tlML = W->tbl[TBL_ML].tableLog;
-        const uint32_t flushBits = tlML + tlOF + tlLL;
-        const uint32_t bsBytes = (totalBits + flushBits + 1 + 7) >> 3;
-        const uint32_t blockBytes = (bsOff - fh - 3) + bsBytes;  // block content size
-        const uint32_t total = fh + 3 + blockBytes + (crc ? 4u : 0u);
-        // blockenc.go:811-817: not smaller than the input => raw block.  Also covers staging overflow.
-        const bool useRaw = (blockBytes >= n) || (total + 8 > PACK_STAGE_BYTES);
-        if (!useRaw) {
-            uint32_t zw = (total + 8 + 3) / 4;
-            for (uint32_t i = tid; i < zw; i += PACK_NT) reinterpret_cast<uint32_t *>(stage)[i] = 0;
-            __syncthreads();
-            if (litMode == 2) {
-                huf_enc_pack(hw, ps->hw.count, lit, four ? 1 : 0, stage, litOff, tid, PACK_NT, 0, &hst);
-            } else if (litMode == 0) {
-                for (uint32_t i = tid; i < nlit; i += PACK_NT) stage[litOff + i] = lit[i];
-            } else if (tid == 0) {
-                stage[litOff] = lit[0];
+        uint32_t litOff, bsStart;   // staging offset of the literal payload, first bit of the sequence bitstream
+        bool hufBits, useRaw;
+        {
+            const uint32_t litMode = lit_mode(hufStatus, payload, nlit), lhSize = lit_header_bytes(litMode, payload, nlit);
+            const uint32_t litBytes = (litMode == 2) ? payload : (litMode == 1 ? 1u : nlit);
+            litOff = fh + 3 + lhSize;
+            const uint32_t seqOff = litOff + litBytes;
+            const uint32_t bsOff = seqOff + nsHdr + 1 + ncSum;
+            const uint32_t bsBytes = (totalBits + tlML + tlOF + tlLL + 1 + 7) >> 3;
+            const uint32_t blockBytes = (bsOff - fh - 3) + bsBytes;  // block content size
+            const uint32_t total = fh + 3 + blockBytes + (crc ? 4u : 0u);
+            // blockenc.go:811-817: not smaller than the input => raw block.  Also covers staging overflow.
+            useRaw = (blockBytes >= n) || (total + 8 > PACK_STAGE_BYTES);
+            hufBits = litMode == 2;
+            bsStart = bsOff * 8 + exBits;
+            if (tid == 0) {
+                ps->litMode = litMode; ps->lhSize = lhSize; ps->litPayload = payload; ps->seqOff = seqOff;
+                ps->total = total; ps->blockBytes = blockBytes; ps->nc0 = nc0; ps->nc1 = nc1;
             }
-            __syncthreads();  // byte stores above must not race the word atomics below
+        }
+        if (!useRaw) {
+            // ------------------------------------------------------------ word-granular phase: the two bitstreams
+            if (hufBits) huf_enc_pack_bits(ps->hw.count, lit, stage, litOff, &hst);
+            B2C_PACK_PHASE(6);
             {
                 BitRun br;
-                br.init(reinterpret_cast<uint32_t *>(stage), bsOff * 8 + exBits);
-#pragma unroll PACK_UNROLL
-                for (uint32_t t = tA; t < tB; t++) {
-                    uint32_t idx = nseq - 1 - t;
-                    uint32_t cl = B2C_LDG(cLL + idx), co = B2C_LDG(cOF + idx), cm = B2C_LDG(cML + idx);
-                    const uint32_t vLL = wlen.get_ll(idx), vML = wlen.get_ml(idx), vOF = B2C_LDG(wof + idx);
-#if PACK_SEQ_COMBINE
-                    if (t) {
-                        // three state flushes (<= 9 bits each) in one append: OF, ML, LL (blockenc.go:757-790)
-                        uint32_t so = B2C_LDG(stbOF + idx), sm = B2C_LDG(stbML + idx), sl = B2C_LDG(stbLL + idx);
-                        const uint32_t no = so >> 12, nm = sm >> 12;
-                        br.add((so & 0xfff) | ((sm & 0xfff) << no) | ((sl & 0xfff) << (no + nm)), no + nm + (sl >> 12));
+                br.init(reinterpret_cast<uint32_t *>(stage), bsStart);
+                for (uint32_t g = gHi; g-- > gLo;) {
+                    const uint2 cl8 = B2C_LDG(cLL + g);
+                    const uint2 co8 = B2C_LDG(cOF + g);
+                    const uint2 cm8 = B2C_LDG(cML + g);
+                    const uint4 sl8 = B2C_LDG(stbLL + g);
+                    const uint4 so8 = B2C_LDG(stbOF + g);
+                    const uint4 sm8 = B2C_LDG(stbML + g);
+                    const uint4 of0 = B2C_LDG(wof + 2 * g), of1 = B2C_LDG(wof + 2 * g + 1);
+                    uint4 ll0, ll1, ml0, ml1;
+                    if (BIG) {
+                        ll0 = B2C_LDG(wll + 2 * g); ll1 = B2C_LDG(wll + 2 * g + 1);
+                        ml0 = B2C_LDG(wml + 2 * g); ml1 = B2C_LDG(wml + 2 * g + 1);
+                    } else {
+                        ll0 = B2C_LDG(wll + g); ml0 = B2C_LDG(wml + g);
+                        ll1 = ml1 = make_uint4(0, 0, 0, 0);
                     }
-                    // extra bits: LL and ML (<= 16 bits each) together, then OF
-                    uint32_t lb = PACK_LLB(cl), mb = PACK_MLB(cm);
-                    br.add((vLL & ((1u << lb) - 1)) | ((vML & ((1u << mb) - 1)) << lb), lb + mb);
-                    br.add(vOF & ((1u << co) - 1), co);
-#else
-                    if (t) {
-                        uint32_t so = B2C_LDG(stbOF + idx), sm = B2C_LDG(stbML + idx), sl = B2C_LDG(stbLL + idx);
-                        br.add(so & 0xfff, so >> 12);
-                        br.add(sm & 0xfff, sm >> 12);
-                        br.add(sl & 0xfff, sl >> 12);
+#pragma unroll
+                    for (int j = 7; j >= 0; j--) {
+                        const uint32_t idx = 8 * g + j;
+                        if (idx < nseq) {
+                            const uint32_t cl = u8_of(cl8, j), co = u8_of(co8, j), cm = u8_of(cm8, j);
+                            const uint32_t vLL = BIG ? u32_of(ll0, ll1, j) : u16_of(ll0, j);
+                            const uint32_t vML = BIG ? u32_of(ml0, ml1, j) : u16_of(ml0, j);
+                            const uint32_t vOF = u32_of(of0, of1, j);
+                            if (idx + 1 < nseq) {
+                                // three state flushes (<= 9 bits each) in one append: OF, ML, LL (blockenc.go:757-790)
+                                const uint32_t so = u16_of(so8, j), sm = u16_of(sm8, j), sl = u16_of(sl8, j);
+                                const uint32_t no = so >> 12, nm = sm >> 12;
+                                br.add((so & 0xfff) | ((sm & 0xfff) << no) | ((sl & 0xfff) << (no + nm)), no + nm + (sl >> 12));
+                            }
+                            // extra bits: LL and ML (<= 16 bits each) together, then OF
+                            const uint32_t lb = PACK_LLB(cl), mb = PACK_MLB(cm);
+                            br.add((vLL & ((1u << lb) - 1)) | ((vML & ((1u << mb) - 1)) << lb), lb + mb);
+                            br.add(vOF & ((1u << co) - 1), co);
+                        }
                     }
-                    uint32_t lb = PACK_LLB(cl), mb = PACK_MLB(cm);
-                    br.add(vLL & ((1u << lb) - 1), lb);
-                    br.add(vML & ((1u << mb) - 1), mb);
-                    br.add(vOF & ((1u << co) - 1), co);
-#endif
                 }
-                if (tB == nseq && tA < tB) {
+                if (gLo == 0 && gHi > 0) {
                     // final states: ml, of, ll (blockenc.go:804-806) + end mark
                     br.add(W->finalState[TBL_ML] & ((1u << tlML) - 1), tlML);
                     br.add(W->finalState[TBL_OF] & ((1u << tlOF) - 1), tlOF);
@@ -641,41 +751,38 @@ B2C_DEV void zstd_pack_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chu
                 }
                 br.finish();
             }
-            __syncthreads();
-            // byte-granular headers (after all word-granular atomics)
-            if (tid == 0) {
-                uint32_t o = 0;
-                if (frame) o = write_frame_header(stage, n, crc);
-                uint32_t bh = lastBit | (2u << 1) | (blockBytes << 3);  // compressed block
-                stage[o++] = (uint8_t)bh; stage[o++] = (uint8_t)(bh >> 8); stage[o++] = (uint8_t)(bh >> 16);
-                // literals header (blockenc.go:153-238)
-                uint64_t lh;
-                if (litMode == 2) {
-                    uint64_t comp = ps->litPayload;
-                    if (lhSize == 3) lh = 2u | ((four ? 1u : 0u) << 2) | ((uint64_t)nlit << 4) | (comp << 14);
-                    else if (lhSize == 4) lh = 2u | (2u << 2) | ((uint64_t)nlit << 4) | (comp << 18);
-                    else lh = 2u | (3u << 2) | ((uint64_t)nlit << 4) | (comp << 22);
-                } else {
-                    uint64_t ty = (litMode == 1) ? 1u : 0u;
-                    if (lhSize == 1) lh = ty | ((uint64_t)nlit << 3);
-                    else if (lhSize == 2) lh = ty | (1u << 2) | ((uint64_t)nlit << 4);
-                    else lh = ty | (3u << 2) | ((uint64_t)nlit << 4);
-                }
-                for (uint32_t k = 0; k < lhSize; k++) stage[o++] = (uint8_t)(lh >> (8 * k));
-                o = seqOff;
+            __syncthreads();  // byte stores below must not race the word atomics above
+            B2C_PACK_PHASE(7);
+            // ------------------------------------------------------------ byte-granular phase: one field per thread
+            const uint32_t litMode = ps->litMode, lhSize = ps->lhSize, payload = ps->litPayload, seqOff = ps->seqOff;
+            const uint32_t total = ps->total, blockBytes = ps->blockBytes, nc0 = ps->nc0, nc1 = ps->nc1;
+            const uint32_t tblOff = seqOff + nsHdr + 1, ncSum = nc0 + nc1 + W->ncountLen[2];
+            if (tid == 0 && frame) write_frame_header(stage, n, crc);
+            if (tid == 32) {
+                const uint32_t bh = lastBit | (2u << 1) | (blockBytes << 3);  // compressed block
+                stage[fh] = (uint8_t)bh; stage[fh + 1] = (uint8_t)(bh >> 8); stage[fh + 2] = (uint8_t)(bh >> 16);
+            }
+            if (tid == 64) {
+                const uint64_t lh = lit_header(litMode, lhSize, nlit, payload, four);
+                for (uint32_t k = 0; k < lhSize; k++) stage[fh + 3 + k] = (uint8_t)(lh >> (8 * k));
+            }
+            if (tid == 96) {
+                uint32_t o = seqOff;
                 if (nseq < 128) stage[o++] = (uint8_t)nseq;
                 else if (nseq < 0x7f00) { stage[o++] = (uint8_t)(128 + (nseq >> 8)); stage[o++] = (uint8_t)nseq; }
                 else { uint32_t v = nseq - 0x7f00; stage[o++] = 255; stage[o++] = (uint8_t)v; stage[o++] = (uint8_t)(v >> 8); }
-                stage[o++] = (uint8_t)((W->mode[TBL_LL] << 6) | (W->mode[TBL_OF] << 4) | (W->mode[TBL_ML] << 2));
-                for (int c = 0; c < 3; c++)
-                    for (uint32_t k = 0; k < W->ncountLen[c]; k++) stage[o++] = W->ncount[c][k];
-                if (crc) {
-                    uint32_t c32 = (uint32_t)W->xxh;
-                    uint32_t e = total - 4;
-                    stage[e] = (uint8_t)c32; stage[e + 1] = (uint8_t)(c32 >> 8); stage[e + 2] = (uint8_t)(c32 >> 16); stage[e + 3] = (uint8_t)(c32 >> 24);
-                }
+                stage[o] = (uint8_t)((W->mode[TBL_LL] << 6) | (W->mode[TBL_OF] << 4) | (W->mode[TBL_ML] << 2));
             }
+            if (crc && tid >= 128 && tid < 132) stage[total - 4 + (tid - 128)] = (uint8_t)((uint32_t)W->xxh >> (8 * (tid - 128)));
+            for (uint32_t k = tid; k < ncSum; k += PACK_NT) {
+                const uint32_t c = k < nc0 ? 0u : (k < nc0 + nc1 ? 1u : 2u);
+                stage[tblOff + k] = W->ncount[c][k - (c == 0 ? 0u : (c == 1 ? nc0 : nc0 + nc1))];
+            }
+            if (litMode == 2) huf_enc_pack_header(hw, four, stage, litOff, tid, PACK_NT);
+            else if (litMode == 0) { for (uint32_t i = tid; i < nlit; i += PACK_NT) stage[litOff + i] = lit[i]; }
+            else if (tid == 0) stage[litOff] = lit[0];
             __syncthreads();
+            B2C_PACK_PHASE(8);
             // one coalesced write-back
             if (total <= P.dst_cap) {
                 if ((reinterpret_cast<uintptr_t>(gdst) & 15) == 0) {
@@ -689,36 +796,32 @@ B2C_DEV void zstd_pack_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chu
                 }
                 if (tid == 0) P.out_sizes[chunk] = (int64_t)total;
             } else if (tid == 0) P.out_sizes[chunk] = -4;  // destination too small
+            B2C_PACK_PHASE(9);
             if (P.dbg_hdr && tid == 0) {
                 uint32_t *d = P.dbg_hdr + (uint64_t)chunk * 4;
                 d[0] = nseq; d[1] = nlit; d[2] = 0; d[3] = litMode;
             }
             return;
         }
-        kind = 1;  // fall through to the raw block
+        kind = 1;  // fall through to the raw block (the bulk copy has landed: every thread waited for it)
     }
 
-    // ---------------------------------------------------------------- raw / RLE block (+ frame)
+    // ---------------------------------------------------------------- raw / RLE block (+ frame), straight to global memory
     {
-        __syncthreads();
-        uint8_t *hdr = stage;
-        if (tid == 0) {
-            uint32_t o = 0;
-            if (frame) o = write_frame_header(hdr, n, crc);
-            uint32_t bh = (kind == 2) ? (lastBit | (1u << 1) | (W->rleLen << 3)) : (lastBit | (0u << 1) | (n << 3));
-            hdr[o++] = (uint8_t)bh; hdr[o++] = (uint8_t)(bh >> 8); hdr[o++] = (uint8_t)(bh >> 16);
-            ps->pos = o;
-        }
-        __syncthreads();
-        const uint32_t hlen = ps->pos;
+        const uint32_t hlen = fh + 3;
         const uint32_t body = (kind == 2) ? 1u : n;
         const bool crcHere = crc && n > 0;
         const uint32_t total = hlen + body + (crcHere ? 4u : 0u);
         if (total <= P.dst_cap) {
-            for (uint32_t i = tid; i < hlen; i += PACK_NT) gdst[i] = hdr[i];
+            if (tid == 0) {
+                if (frame) write_frame_header(gdst, n, crc);
+                const uint32_t bh = (kind == 2) ? (lastBit | (1u << 1) | (W->rleLen << 3)) : (lastBit | (0u << 1) | (n << 3));
+                gdst[fh] = (uint8_t)bh; gdst[fh + 1] = (uint8_t)(bh >> 8); gdst[fh + 2] = (uint8_t)(bh >> 16);
+                P.out_sizes[chunk] = (int64_t)total;
+            }
+            const uint8_t *gsrc = chunk_src(P, chunk);
             for (uint32_t i = tid; i < body; i += PACK_NT) gdst[hlen + i] = gsrc[i];
             if (crcHere && tid < 4) gdst[hlen + body + tid] = (uint8_t)((uint32_t)W->xxh >> (8 * tid));
-            if (tid == 0) P.out_sizes[chunk] = (int64_t)total;
         } else if (tid == 0) P.out_sizes[chunk] = -4;
         if (P.dbg_hdr && tid == 0) {
             uint32_t *d = P.dbg_hdr + (uint64_t)chunk * 4;

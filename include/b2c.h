@@ -165,8 +165,9 @@ B2C_API int b2c_zstd_encode_device_debug(b2c_ctx *ctx, int level, int flags, con
                                          int64_t *d_out_sizes, uint32_t nchunks, uint32_t *d_dbg_hdr,
                                          uint32_t *d_dbg_seqs, uint8_t *d_dbg_lits, uint32_t dbg_seq_cap, void *stream);
 
-/* Profiling hook: like b2c_zstd_encode_device (all chunks size_all bytes) but thread 0 of every CTA also
- * stores clock64() at 15 phase boundaries into d_cycles[chunk][16] (tools/phase_times.py). */
+/* Profiling hook: like b2c_zstd_encode_device (level 1, all chunks size_all bytes) but lane 0 of every warp of the
+ * parse and pack kernels also stores clock64() at their phase boundaries into d_cycles[chunk][16][32]: columns 0-15
+ * the parse's warps (tools/phase_times.py), 16-31 the pack kernel's (tools/pack_phase_times.py). */
 B2C_API int b2c_zstd_encode_device_timed(b2c_ctx *ctx, int flags, const void *d_src, size_t src_stride,
                                          uint32_t size_all, void *d_dst, size_t dst_stride, int64_t *d_out_sizes,
                                          uint32_t nchunks, unsigned long long *d_cycles, void *stream);

@@ -28,7 +28,7 @@ def main():
                                               outs.data_ptr(), n, cyc.data_ptr(), None)
         check(rc, enc._ctx)
         torch.cuda.synchronize()
-    c = cyc.cpu().numpy().astype(np.int64)       # [n, 16, 32]: arrival of warp w at stamp k (0 where the warp does not exist)
+    c = cyc.cpu().numpy().astype(np.int64)[:, :, :16]   # [n, 16, 16]: arrival of warp w at stamp k (0 where the warp does not exist); columns 16.. are the pack kernel's
     nw = int((c[0, 0] != 0).sum())
     c = c[:, :, :nw]
     order, names = ORDER, NAMES
