@@ -24,7 +24,7 @@
 #include "b2c_lz4_cvt.cuh"
 
 #ifndef TABLES_CTAS_PER_SM
-#define TABLES_CTAS_PER_SM 8   // K2: resident CTAs per SM (19 KB static shared memory, 56 registers x 128 threads each)
+#define TABLES_CTAS_PER_SM TABLES_MIN_CTAS   // K2: resident CTAs per SM (44 KB static shared memory each)
 #endif
 
 using namespace b2c;
@@ -544,7 +544,8 @@ static int launch_encode(b2c_ctx *ctx, int level, int flags, const void *d_src, 
             ctx->launches += 2;
         }
         PEV(3);
-        const unsigned g2 = sms * TABLES_CTAS_PER_SM < m ? sms * TABLES_CTAS_PER_SM : m;
+        const unsigned m2 = (m + TABLES_NW - 1) / TABLES_NW;     // K2 takes one chunk per warp at a time
+        const unsigned g2 = sms * TABLES_CTAS_PER_SM < m2 ? sms * TABLES_CTAS_PER_SM : m2;
         b2c_zstd_tables_kernel<<<g2, TABLES_NT, 0, st>>>(P);
         PEV(4);
         b2c_zstd_chains_kernel<<<(m + 31) / 32, CHAIN_NT + ((wantXxh && ctx->enc_fused_xxh) ? CHAIN_XXH_NT : 0), CHAIN_SMEM_BYTES, st>>>(P);

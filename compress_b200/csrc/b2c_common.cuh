@@ -27,6 +27,12 @@ namespace b2c {
 B2C_DEV unsigned lane_id() { return threadIdx.x & 31; }
 B2C_DEV unsigned warp_id() { return threadIdx.x >> 5; }
 B2C_DEV uint32_t highbit32(uint32_t v) { return 31u - (uint32_t)__clz((int)v); }  // v != 0
+// Profiling stamp: lane 0 stores clock64 at row[k] (nothing without a row, and nothing in the emulator build).
+B2C_DEV void stamp_clock(unsigned long long *row, int k) {
+#ifndef B2C_EMU
+    if (row && lane_id() == 0) row[k] = (unsigned long long)clock64();
+#endif
+}
 
 // Named barrier over a warp-multiple subset of the CTA (id 1..15; 0 is __syncthreads).
 B2C_DEV void bar_sync(int id, int nthreads) {

@@ -4,9 +4,9 @@
 //   zstd/fse_encoder.go:102-204 (buildCTable), :259-427 (normalizeCount/2),
 //   :429-455 (optimalTableLog), :488-598 (writeCount), :603-672 (bitCost/approxSize)
 //   fse/compress.go (same arithmetic, used for huff0 weight tables).
-// Tables here are tiny (<= 64 symbols, <= 256 states); each table is built by a
-// single thread while other warps build the other tables.  All results are
-// bit-exact with the oracle (tests/test_entropy_parity.py).
+// Tables here are tiny (<= 64 symbols, <= 256 states); each table is built by one
+// warp (normalisation, table fill and size estimates over its lanes; the NCount and
+// the predefined tables on one thread).  All results are bit-exact with the oracle.
 #pragma once
 #include "b2c_common.cuh"
 
@@ -81,37 +81,53 @@ B2C_DEV int fse_normalize2(const uint32_t *count, uint32_t symbolLen, uint32_t l
     return 0;
 }
 
+// normalizeCount by one warp (symbolLen <= 64: symbols lane and lane + 32); every lane calls and gets the same result.
+// The serial loop's running largest (first symbol with the highest probability) is a warp arg-max with the same tie
+// rule; the rare fall-back to normalizeCount2 runs on lane 0.
 B2C_DEV int fse_normalize(const uint32_t *count, uint32_t symbolLen, uint32_t length, uint32_t tableLog,
-                          int16_t *norm) {
+                          int16_t *norm, unsigned lane) {
     const uint32_t rtb[8] = {0, 473195, 504333, 520860, 550000, 700000, 750000, 830000};
-    uint64_t scale = 62 - (uint64_t)tableLog;
-    uint64_t step = (1ull << 62) / (uint64_t)length;
-    uint64_t vStep = 1ull << (scale - 20);
-    int16_t stillToDistribute = (int16_t)(1 << tableLog);
-    uint32_t largest = 0;
-    int16_t largestP = 0;
-    uint32_t lowThreshold = length >> tableLog;
-    for (uint32_t i = 0; i < symbolLen; i++) {
-        uint32_t cnt = count[i];
-        if (cnt == 0) { norm[i] = 0; continue; }
-        if (cnt <= lowThreshold) {
-            norm[i] = -1;
-            stillToDistribute--;
-        } else {
-            int16_t proba = (int16_t)(((uint64_t)cnt * step) >> scale);
+    const uint64_t scale = 62 - (uint64_t)tableLog;
+    const uint64_t step = (1ull << 62) / (uint64_t)length;
+    const uint64_t vStep = 1ull << (scale - 20);
+    const uint32_t lowThreshold = length >> tableLog;
+    int used = 0;           // states this lane's symbols take
+    uint32_t key = 0;       // proba << 8 | (255 - symbol) of this lane's best symbol (0: none)
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const uint32_t i = lane + 32u * (uint32_t)h;
+        if (i >= symbolLen) continue;
+        const uint32_t cnt = count[i];
+        int proba = 0;
+        if (cnt == 0) proba = 0;
+        else if (cnt <= lowThreshold) { proba = -1; used += 1; }
+        else {
+            proba = (int)(((uint64_t)cnt * step) >> scale);
             if (proba < 8) {
-                uint64_t restToBeat = vStep * (uint64_t)rtb[proba];
-                uint64_t v = (uint64_t)cnt * step - ((uint64_t)proba << scale);
+                const uint64_t restToBeat = vStep * (uint64_t)rtb[proba];
+                const uint64_t v = (uint64_t)cnt * step - ((uint64_t)proba << scale);
                 if (v > restToBeat) proba++;
             }
-            if (proba > largestP) { largestP = proba; largest = i; }
-            norm[i] = proba;
-            stillToDistribute = (int16_t)(stillToDistribute - proba);
+            used += proba;
+            const uint32_t k = ((uint32_t)proba << 8) | (255u - i);
+            if (proba > 0 && k > key) key = k;
         }
+        norm[i] = (int16_t)proba;
     }
-    if ((int16_t)(-stillToDistribute) >= (int16_t)(norm[largest] >> 1))
-        return fse_normalize2(count, symbolLen, length, tableLog, norm);
-    norm[largest] = (int16_t)(norm[largest] + stillToDistribute);
+    const int stillToDistribute = (1 << tableLog) - (int)warp_sum((uint32_t)used);
+    key = warp_max(key);
+    const uint32_t largest = key ? 255u - (key & 255u) : 0u;
+    __syncwarp();
+    const int largestP = key ? (int)(key >> 8) : (int)norm[0];   // norm[largest]
+    if (-stillToDistribute >= (largestP >> 1)) {
+        int r = 0;
+        if (lane == 0) r = fse_normalize2(count, symbolLen, length, tableLog, norm);
+        r = __shfl_sync(FULLMASK, r, 0);
+        __syncwarp();
+        return r;
+    }
+    if (lane == 0) norm[largest] = (int16_t)(largestP + stillToDistribute);
+    __syncwarp();
     return 0;
 }
 
@@ -333,27 +349,32 @@ B2C_DEV uint32_t fse_init_state(const FseCTable *ct, uint32_t sym) {
     return ct->stateTable[lu];
 }
 
-// bitCost / approxSize (hist length = histLen)
-B2C_DEV uint32_t fse_approx_size(const FseCTable *s, const uint32_t *hist, uint32_t histLen) {
+// bitCost / approxSize (hist length = histLen <= 64) by one warp: symbols lane and lane + 32, a warp sum (the 32-bit
+// sum wraps the same in any order).  Every lane calls and gets the same result.
+B2C_DEV uint32_t fse_approx_size(const FseCTable *s, const uint32_t *hist, uint32_t histLen, unsigned lane) {
     if (s->symbolLen < histLen) return 0xffffffffu;
     if (s->useRLE) return 0xffffffffu;
     const uint32_t kAcc = 8;
-    uint32_t badCost = (s->tableLog + 1) << kAcc;
+    const uint32_t badCost = (s->tableLog + 1) << kAcc;
     uint32_t cost = 0;
-    for (uint32_t i = 0; i < histLen; i++) {
-        if (hist[i] == 0) continue;
-        if (s->norm[i] == 0) return 0xffffffffu;
-        uint32_t dnb = s->deltaNbBits[i];
-        uint32_t minNbBits = dnb >> 16;
-        uint32_t threshold = (minNbBits + 1) << 16;
-        uint32_t tableSize = 1u << s->tableLog;
-        uint32_t deltaFromThreshold = threshold - (dnb + tableSize);
-        uint32_t normalizedDelta = (deltaFromThreshold << kAcc) >> s->tableLog;
-        uint32_t bc = (minNbBits + 1) * (1u << kAcc) - normalizedDelta;
-        if (bc > badCost) return 0xffffffffu;
+    bool bad = false;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const uint32_t i = lane + 32u * (uint32_t)h;
+        if (i >= histLen || hist[i] == 0) continue;
+        if (s->norm[i] == 0) { bad = true; continue; }
+        const uint32_t dnb = s->deltaNbBits[i];
+        const uint32_t minNbBits = dnb >> 16;
+        const uint32_t threshold = (minNbBits + 1) << 16;
+        const uint32_t tableSize = 1u << s->tableLog;
+        const uint32_t deltaFromThreshold = threshold - (dnb + tableSize);
+        const uint32_t normalizedDelta = (deltaFromThreshold << kAcc) >> s->tableLog;
+        const uint32_t bc = (minNbBits + 1) * (1u << kAcc) - normalizedDelta;
+        if (bc > badCost) { bad = true; continue; }
         cost += hist[i] * bc;
     }
-    return cost >> kAcc;
+    if (__any_sync(FULLMASK, bad)) return 0xffffffffu;
+    return warp_sum(cost) >> kAcc;
 }
 
 }  // namespace b2c

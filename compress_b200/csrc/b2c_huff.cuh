@@ -8,7 +8,8 @@
 // One CTA cooperates on one block of literals:
 //   histogram   : per-warp private bins, lanes merged with match.any (no shared atomics)
 //   table build : rank-sort by all threads (same order as huffSort: count desc, symbol asc),
-//                 two-queue tree + setMaxHeight by one lane (<= 255 steps, bit-exact tie-breaks)
+//                 two-queue tree by one lane (<= 255 steps, bit-exact tie-breaks), depths and the table
+//                 description by one warp
 //   encode      : code-length suffix sums (block scan) then every thread packs its own
 //                 contiguous bit range of the 4 backward streams straight into the staging buffer.
 // Output bytes are identical to the oracle's for the same literals.
@@ -149,35 +150,11 @@ B2C_DEV uint32_t huf_set_max_height(HufWork *hw, int lastNonNull, uint32_t maxNb
     return maxNbBits;
 }
 
-// FSE-compress the weights (fse.Compress with TableLog 6 and a supplied histogram).
-// Serial, one thread.  Returns bytes written to out or -1 (=> caller falls back to 4-bit weights).
-B2C_DEV int huf_fse_compress_weights(HufWork *hw, const uint8_t *in, uint32_t n, const uint32_t *hist,
-                                     uint32_t symbolLen, uint32_t maxCount, uint8_t *out /* >= 300 bytes */) {
-    if (n <= 1) return -1;
-    if (maxCount == n) return -1;                      // ErrUseRLE
-    if (maxCount == 1 || maxCount < (n >> 7)) return -1;  // ErrIncompressible
-    // optimalTableLog (fse/compress.go:483-508) with TableLog = 6
-    uint8_t tableLog = 6;
-    {
-        uint32_t minBitsSrc = fse_hb(n - 1) + 1;
-        uint32_t minBitsSymbols = fse_hb(symbolLen - 1) + 2;
-        uint8_t minBits = (uint8_t)(minBitsSrc < minBitsSymbols ? minBitsSrc : minBitsSymbols);
-        uint8_t maxBitsSrc = (uint8_t)((uint8_t)fse_hb(n - 1) - 2);
-        if (maxBitsSrc < tableLog) tableLog = maxBitsSrc;
-        if (minBits > tableLog) tableLog = minBits;
-        if (tableLog < 5) tableLog = 5;
-        if (tableLog > 12) tableLog = 12;
-    }
-    FseCTable *ct = &hw->wct;
-    ct->symbolLen = symbolLen; ct->tableLog = tableLog; ct->useRLE = 0;
-    for (uint32_t i = 0; i < FSE_MAX_SYM; i++) ct->norm[i] = 0;
-    if (fse_normalize(hist, symbolLen, n, tableLog, ct->norm)) return -1;
-    int hdr = fse_write_ncount(ct->norm, symbolLen, tableLog, out);
-    if (hdr < 0) return -1;
-    if (fse_build_ctable(ct)) return -1;
-    if (n <= 2) return -1;
+// The 2-state encode of huf_fse_compress_weights (one thread): the weights' bitstream after the hdr NCount bytes.
+B2C_DEV int huf_fse_encode_weights(const FseCTable *ct, const uint8_t *in, uint32_t n, uint32_t tableLog, uint8_t *out,
+                                   uint32_t hdr) {
     // 2-state backward encode (fse/compress.go:121-205); plain LSB-first concatenation
-    uint64_t acc = 0; uint32_t nacc = 0; uint32_t o = (uint32_t)hdr;
+    uint64_t acc = 0; uint32_t nacc = 0; uint32_t o = hdr;
 #define WADD(val, nb)                                                                                  \
     do {                                                                                               \
         uint32_t nb__ = (nb);                                                                          \
@@ -225,12 +202,50 @@ B2C_DEV int huf_fse_compress_weights(HufWork *hw, const uint8_t *in, uint32_t n,
     return (int)o;
 }
 
+// FSE-compress the weights (fse.Compress with TableLog 6 and a supplied histogram) by one warp: normalisation and
+// table fill by all lanes, the NCount and the 2-state encode on lane 0.  Every lane calls and gets the same result:
+// bytes written to out or -1 (=> caller falls back to 4-bit weights).  Uses hw->nparent as table-fill scratch.
+B2C_DEV int huf_fse_compress_weights(HufWork *hw, const uint8_t *in, uint32_t n, const uint32_t *hist,
+                                     uint32_t symbolLen, uint32_t maxCount, uint8_t *out /* >= 300 bytes */,
+                                     unsigned lane) {
+    if (n <= 1) return -1;
+    if (maxCount == n) return -1;                      // ErrUseRLE
+    if (maxCount == 1 || maxCount < (n >> 7)) return -1;  // ErrIncompressible
+    // optimalTableLog (fse/compress.go:483-508) with TableLog = 6
+    uint8_t tableLog = 6;
+    {
+        uint32_t minBitsSrc = fse_hb(n - 1) + 1;
+        uint32_t minBitsSymbols = fse_hb(symbolLen - 1) + 2;
+        uint8_t minBits = (uint8_t)(minBitsSrc < minBitsSymbols ? minBitsSrc : minBitsSymbols);
+        uint8_t maxBitsSrc = (uint8_t)((uint8_t)fse_hb(n - 1) - 2);
+        if (maxBitsSrc < tableLog) tableLog = maxBitsSrc;
+        if (minBits > tableLog) tableLog = minBits;
+        if (tableLog < 5) tableLog = 5;
+        if (tableLog > 12) tableLog = 12;
+    }
+    FseCTable *ct = &hw->wct;
+    if (lane == 0) { ct->symbolLen = symbolLen; ct->tableLog = tableLog; ct->useRLE = 0; }
+    ct->norm[lane] = 0; ct->norm[lane + 32] = 0;
+    __syncwarp();
+    if (fse_normalize(hist, symbolLen, n, tableLog, ct->norm, lane)) return -1;
+    int hdr = 0;
+    if (lane == 0) hdr = fse_write_ncount(ct->norm, symbolLen, tableLog, out);
+    hdr = __shfl_sync(FULLMASK, hdr, 0);
+    if (hdr < 0) return -1;
+    if (fse_build_ctable_warp(ct, hw->nparent, lane)) return -1;
+    if (n <= 2) return -1;
+    int o = 0;
+    if (lane == 0) o = huf_fse_encode_weights(ct, in, n, tableLog, out, (uint32_t)hdr);
+    o = __shfl_sync(FULLMASK, o, 0);
+    __syncwarp();
+    return o;
+}
 // ---------------------------------------------------------------- table build (staged)
 // Stage A (all threads of the group): symbolLen / maxCount / early outs, then the rank sort.
 //   caller barriers: after huf_bt_stats, after huf_bt_sort.
-// Stage B (one thread): tree, depths, setMaxHeight, valPerRank.
+// Stage B (one warp): tree merge (lane 0), depths, setMaxHeight, valPerRank.
 // Stage C (all threads): ctBits then ctVal (barrier between the two halves is inside).
-// Stage D (one thread): serialise the table (FSE-compressed or 4-bit weights).
+// Stage D (one warp): serialise the table (FSE-compressed or 4-bit weights).
 B2C_DEV void huf_bt_stats(HufWork *hw, uint32_t n, unsigned tid) {
     if (tid < 32) {
         uint32_t m = 0, sl = 0;
@@ -296,14 +311,13 @@ B2C_DEV void huf_bt_sort(HufWork *hw, unsigned tid, unsigned nthreads) {
     }
     for (unsigned s = tid; s < 256; s += nthreads) hw->ctBits[s] = 0;
 }
-B2C_DEV void huf_bt_tree(HufWork *hw, uint32_t n) {
+// Tree merge (one thread): parents of every node, nonNullRank.
+B2C_DEV void huf_bt_merge(HufWork *hw) {
     uint32_t symbolLen = hw->symbolLen;
     uint32_t *cnt0 = hw->ncount;      // huffNode0
     uint32_t *cnt = hw->ncount + 1;   // huffNode
     uint16_t *par0 = hw->nparent;
     uint16_t *par = hw->nparent + 1;
-    uint8_t *nb = hw->nbits + 1;
-    uint32_t tl = huf_optimal_tablelog(11, n, symbolLen);
     int startNode = (int)symbolLen;
     int nonNullRank = (int)symbolLen - 1;
     int nodeNb = startNode;
@@ -330,22 +344,86 @@ B2C_DEV void huf_bt_tree(HufWork *hw, uint32_t n) {
         par0[n1 + 1] = (uint16_t)nodeNb; par0[n2 + 1] = (uint16_t)nodeNb;
         nodeNb++;
     }
-    nb[nodeRoot] = 0;
-    for (int k = nodeRoot - 1; k >= startNode; k--) nb[k] = (uint8_t)(nb[par[k]] + 1);
-    for (int k = 0; k <= nonNullRank; k++) nb[k] = (uint8_t)(nb[par[k]] + 1);
-    uint32_t maxNbBits = huf_set_max_height(hw, nonNullRank, tl);
-    hw->tableLog = maxNbBits;
     hw->nonNullRank = (uint32_t)nonNullRank;
-    // valPerRank (compress.go:536-550) -> scan[] for the parallel assignment
-    uint16_t nbPerRank[HUF_TABLELOG_MAX + 2];
-    for (int i = 0; i < HUF_TABLELOG_MAX + 2; i++) nbPerRank[i] = 0;
-    for (int i = 0; i <= nonNullRank; i++) nbPerRank[nb[i]]++;
-    uint16_t mn = 0;
-    for (uint32_t r = maxNbBits; r > 0; r--) {
-        hw->scan[r] = mn;
-        mn = (uint16_t)(mn + nbPerRank[r]);
-        mn >>= 1;
+}
+// Depths by one warp (every lane calls): nbBits of the leaves 0..nonNullRank and of the internal nodes, by pointer
+// jumping over the parent links (a node's depth doubles its reach every round: at most 8 rounds for 255 leaves).  The
+// parent links are consumed (nparent holds jumped links afterwards).
+B2C_DEV void huf_bt_depths(HufWork *hw, unsigned lane) {
+    constexpr int PER = 16;                               // <= 510 nodes, 16 per lane
+    const uint32_t startNode = hw->symbolLen, nnr = hw->nonNullRank, nodeRoot = startNode + nnr - 1;
+    const uint32_t nNodes = 2 * nnr;                      // leaves 0..nnr, internal nodes startNode..nodeRoot-1
+    uint16_t *par = hw->nparent + 1;
+    uint8_t *nb = hw->nbits + 1;
+    uint32_t pd[PER];                                     // link << 8 | distance to it
+#pragma unroll
+    for (int j = 0; j < PER; j++) {
+        const uint32_t i = lane + 32u * (uint32_t)j;
+        const uint32_t k = i <= nnr ? i : startNode + (i - nnr - 1);
+        pd[j] = nodeRoot << 8 | 1u;
+        if (i < nNodes) { pd[j] = (uint32_t)par[k] << 8 | 1u; nb[k] = 1; }
     }
+    if (lane == 0) { par[nodeRoot] = (uint16_t)nodeRoot; nb[nodeRoot] = 0; }
+    __syncwarp();
+    for (;;) {
+        uint32_t t[PER];
+#pragma unroll
+        for (int j = 0; j < PER; j++) {
+            const uint32_t p = pd[j] >> 8;
+            t[j] = (p != nodeRoot) ? (uint32_t)nb[p] | ((uint32_t)par[p] << 8) : 0u;
+        }
+        __syncwarp();
+        bool more = false;
+#pragma unroll
+        for (int j = 0; j < PER; j++) {
+            if ((pd[j] >> 8) == nodeRoot) continue;
+            const uint32_t i = lane + 32u * (uint32_t)j;
+            const uint32_t k = i <= nnr ? i : startNode + (i - nnr - 1);
+            pd[j] = (t[j] & ~255u) | ((pd[j] & 255u) + (t[j] & 255u));   // depths stay below 256
+            nb[k] = (uint8_t)pd[j]; par[k] = (uint16_t)(pd[j] >> 8);
+            more |= (pd[j] >> 8) != nodeRoot;
+        }
+        __syncwarp();
+        if (!__any_sync(FULLMASK, more)) break;
+    }
+}
+// setMaxHeight (lane 0; it returns at once unless a code is longer than maxNbBits), then valPerRank (compress.go:536-550)
+// -> scan[] for the parallel assignment, with the per-length counts from ballots.  Every lane calls.
+B2C_DEV void huf_bt_ranks(HufWork *hw, uint32_t n, unsigned lane) {
+    const uint32_t nnr = hw->nonNullRank;
+    const uint8_t *nb = hw->nbits + 1;
+    uint32_t maxNbBits = 0;
+    if (lane == 0) maxNbBits = huf_set_max_height(hw, (int)nnr, huf_optimal_tablelog(11, n, hw->symbolLen));
+    maxNbBits = __shfl_sync(FULLMASK, maxNbBits, 0);
+    __syncwarp();
+    uint32_t nbPerRank[HUF_TABLELOG_MAX + 1];
+#pragma unroll
+    for (int r = 0; r <= HUF_TABLELOG_MAX; r++) nbPerRank[r] = 0;
+    for (uint32_t i0 = 0; i0 <= nnr; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        const uint32_t v = i <= nnr ? nb[i] : 0u;
+#pragma unroll
+        for (int r = 1; r <= HUF_TABLELOG_MAX; r++) nbPerRank[r] += (uint32_t)__popc(__ballot_sync(FULLMASK, v == (uint32_t)r));
+    }
+    if (lane == 0) {
+        hw->tableLog = maxNbBits;
+        uint16_t mn = 0;
+#pragma unroll
+        for (int r = HUF_TABLELOG_MAX; r > 0; r--) {
+            if ((uint32_t)r > maxNbBits) continue;
+            hw->scan[r] = mn;
+            mn = (uint16_t)(mn + nbPerRank[r]);
+            mn >>= 1;
+        }
+    }
+    __syncwarp();
+}
+// The whole code-length build by one warp (every lane calls).
+B2C_DEV void huf_bt_tree(HufWork *hw, uint32_t n, unsigned lane) {
+    if (lane == 0) huf_bt_merge(hw);
+    __syncwarp();
+    huf_bt_depths(hw, lane);
+    huf_bt_ranks(hw, n, lane);
 }
 B2C_DEV void huf_bt_bits(HufWork *hw, unsigned tid, unsigned nthreads) {
     for (unsigned i = tid; i <= hw->nonNullRank; i += nthreads) hw->ctBits[hw->nsym[1 + i]] = hw->nbits[1 + i];
@@ -383,42 +461,63 @@ B2C_DEV void huf_bt_vals(HufWork *hw, unsigned tid, unsigned nthreads) {
         hw->ctVal[s] = (uint16_t)v;
     }
 }
-// cTable.write (huff0.go:180-247), one thread
-B2C_DEV void huf_bt_write(HufWork *hw) {
-    uint32_t symbolLen = hw->symbolLen;
-    uint32_t huffLog = hw->tableLog;
-    uint8_t maxSymbolValue = (uint8_t)(symbolLen - 1);
+// cTable.write (huff0.go:180-247) by one warp (every lane calls): weights and their histogram from ballots, the FSE
+// compression of huf_fse_compress_weights, or the 4-bit form.
+B2C_DEV void huf_bt_write(HufWork *hw, unsigned lane) {
+    const uint32_t symbolLen = hw->symbolLen;
+    const uint32_t huffLog = hw->tableLog;
+    const uint32_t maxSymbolValue = symbolLen - 1;
     uint32_t hist[16];
-    for (int i = 0; i < 16; i++) hist[i] = 0;
-    for (uint32_t k = 0; k < maxSymbolValue; k++) {
-        uint32_t nbk = hw->ctBits[k];
-        uint8_t wv = nbk ? (uint8_t)((huffLog + 1 - nbk) & 15) : 0;
-        hw->weight[k] = wv;
-        hist[wv]++;
+#pragma unroll
+    for (int v = 0; v < 16; v++) hist[v] = 0;
+    for (uint32_t k0 = 0; k0 < maxSymbolValue; k0 += 32) {
+        const uint32_t k = k0 + lane;
+        const bool valid = k < maxSymbolValue;
+        uint32_t wv = 16;
+        if (valid) {
+            const uint32_t nbk = hw->ctBits[k];
+            wv = nbk ? ((huffLog + 1 - nbk) & 15) : 0;
+            hw->weight[k] = (uint8_t)wv;
+        }
+#pragma unroll
+        for (int v = 0; v < 16; v++) hist[v] += (uint32_t)__popc(__ballot_sync(FULLMASK, wv == (uint32_t)v));
     }
-    int done = 0;
+    uint32_t *whist = hw->scan + 16;      // scan[] is free once the code values are assigned
+    if (lane < 16) {
+        uint32_t h = 0;
+#pragma unroll
+        for (int v = 0; v < 16; v++) if (lane == (unsigned)v) h = hist[v];
+        whist[lane] = h;
+    }
+    __syncwarp();
+    bool done = false;
     if (maxSymbolValue >= 2) {
         uint32_t huffMaxCnt = 0, huffMax = 0;
-        for (uint32_t i = 0; i < 16; i++) {
-            if (!hist[i]) continue;
-            huffMax = i;
-            if (hist[i] > huffMaxCnt) huffMaxCnt = hist[i];
+#pragma unroll
+        for (int v = 0; v < 16; v++) {
+            if (!hist[v]) continue;
+            huffMax = (uint32_t)v;
+            if (hist[v] > huffMaxCnt) huffMaxCnt = hist[v];
         }
         // tableDesc[0] is the size byte; the FSE payload goes to tableDesc+1..
-        int b = huf_fse_compress_weights(hw, hw->weight, maxSymbolValue, hist, huffMax + 1, huffMaxCnt,
-                                         hw->tableDesc + 1);
-        if (b >= 0 && b < (int)(symbolLen >> 1)) { hw->tableDesc[0] = (uint8_t)b; hw->tableDescLen = (uint32_t)b + 1; done = 1; }
-    }
-    if (!done) {
-        if (maxSymbolValue > 128) { hw->status = HUF_INCOMPRESSIBLE; }
-        else {
-            uint32_t o = 0;
-            hw->tableDesc[o++] = (uint8_t)(128 | (maxSymbolValue - 1));
-            hw->weight[maxSymbolValue] = 0;
-            for (uint32_t k = 0; k < maxSymbolValue; k += 2) hw->tableDesc[o++] = (uint8_t)((hw->weight[k] << 4) | hw->weight[k + 1]);
-            hw->tableDescLen = o;
+        const int b = huf_fse_compress_weights(hw, hw->weight, maxSymbolValue, whist, huffMax + 1, huffMaxCnt,
+                                               hw->tableDesc + 1, lane);
+        if (b >= 0 && b < (int)(symbolLen >> 1)) {
+            if (lane == 0) { hw->tableDesc[0] = (uint8_t)b; hw->tableDescLen = (uint32_t)b + 1; }
+            done = true;
         }
     }
+    if (!done) {
+        if (maxSymbolValue > 128) { if (lane == 0) hw->status = HUF_INCOMPRESSIBLE; }
+        else {
+            if (lane == 0) { hw->weight[maxSymbolValue] = 0; hw->tableDesc[0] = (uint8_t)(128 | (maxSymbolValue - 1)); }
+            __syncwarp();
+            const uint32_t nb = (maxSymbolValue + 1) >> 1;
+            for (uint32_t j = lane; j < nb; j += 32) hw->tableDesc[1 + j] = (uint8_t)((hw->weight[2 * j] << 4) | hw->weight[2 * j + 1]);
+            if (lane == 0) hw->tableDescLen = 1 + nb;
+        }
+    }
+    __syncwarp();
 }
 // Convenience: whole build with barriers (all threads of the group call).
 // Code lengths and code values only (stages A-C): ctBits / ctVal / tableLog / symbolLen; hw->status on the early outs.
@@ -429,7 +528,7 @@ B2C_DEV void huf_build_codes(HufWork *hw, uint32_t n, unsigned tid, unsigned nth
     if (hw->status != HUF_OK) return;
     huf_bt_sort(hw, tid, nthreads);
     HSYNC();
-    if (tid == 0) huf_bt_tree(hw, n);
+    if (tid < 32) huf_bt_tree(hw, n, tid);
     HSYNC();
     huf_bt_bits(hw, tid, nthreads);
     HSYNC();
@@ -440,7 +539,7 @@ B2C_DEV void huf_build_codes(HufWork *hw, uint32_t n, unsigned tid, unsigned nth
 B2C_DEV void huf_build_table(HufWork *hw, uint32_t n, unsigned tid, unsigned nthreads, int bar_id) {
     huf_build_codes(hw, n, tid, nthreads, bar_id);
     if (hw->status != HUF_OK) return;
-    if (tid == 0) huf_bt_write(hw);
+    if (tid < 32) huf_bt_write(hw, tid);
     group_sync(bar_id, (int)nthreads);
 }
 

@@ -6,13 +6,8 @@
 //   zstd/seqenc.go:48-112 (llCode/mlCode/ofCode + extra-bit tables)
 //   zstd/fse_encoder.go (normalizeCount/buildCTable/writeCount/approxSize, via b2c_fse.cuh)
 //   zstd/fse_predefined.go:118-156 (default distributions)
-// The three tANS state chains are serial in the reference.  Here each chain is
-// cut into 32 segments walked by the 32 lanes of one warp: a lane first runs a
-// short warm-up over the symbols preceding its segment (tANS encoder states
-// forget their past at ~nbBits per step), then its segment; lanes whose assumed
-// start state disagrees with the predecessor's verified final state re-run, so
-// the result is always the exact serial chain.  Bits are then packed by all
-// threads at prefix-summed offsets.  Output bytes equal the oracle's.
+// Code tables, the predefined tables and the per-block table build (K2); the state chains themselves are walked by
+// zstd_chains_block (b2c_zstd_enc.cuh).  Output bytes equal the oracle's.
 #pragma once
 #include "b2c_common.cuh"
 #include "b2c_fse.cuh"
@@ -20,23 +15,21 @@
 namespace b2c {
 
 enum { TBL_LL = 0, TBL_OF = 1, TBL_ML = 2 };
-constexpr int SEQ_WARMUP = 24;
 constexpr uint32_t SEQ_TABLE_ERR = 0xffffffffu;  // ncountLen marker: table construction failed
 
+// The predefined tables (fse_predefined.go), built once per CTA and read by every warp's mode decision.
 struct SeqWork {
-    FseCTable cur[3];
     FseCTable predef[3];
-    uint32_t hist[3][64];
-    uint32_t maxSym[3];
-    uint32_t mode[3];          // 0 predefined, 1 RLE, 2 FSE
-    uint32_t used[3];          // 0 -> predef[i], 1 -> cur[i]
-    uint8_t ncount[3][96];
-    uint32_t ncountLen[3];
-    uint32_t finalState[3];
-    uint32_t scan[40];
-    uint32_t totalBits;
-    int32_t err;
-    uint16_t fseScratch[3][200];   // fse_build_ctable_warp
+};
+// One warp's scratch for building one sequence table.
+struct SeqTableWork {
+    FseCTable cur;
+    uint32_t hist[64];
+    uint32_t mode;             // 0 predefined, 1 RLE, 2 FSE
+    uint32_t used;             // 0 -> the predefined table, 1 -> cur
+    uint32_t ncountLen;
+    uint8_t ncount[96];
+    uint16_t fseScratch[200];  // fse_build_ctable_warp
 };
 
 B2C_DEV uint32_t seq_ll_code(uint32_t litLength) {
@@ -116,17 +109,20 @@ B2C_DEV uint32_t seq_optimal_tablelog(uint32_t length, uint32_t symbolLen) {
     return tableLog;
 }
 
-// One warp builds table `which` from sw->hist[which] (fresh block: no previous tables); every lane calls.
-// firstCode = code of sequence 0 (setRLE uses b.sequences[0]).  Lane 0 runs the serial steps (normalisation, size
-// estimates, NCount), the table itself is filled by all lanes.
-B2C_DEV void seq_build_table(SeqWork *sw, int which, uint32_t nseq, uint32_t firstCode, unsigned lane) {
-    FseCTable *ct = &sw->cur[which];
-    const uint32_t *hist = sw->hist[which];
-    const uint32_t symbolLen = sw->maxSym[which] + 1;
+// One warp builds a table from st->hist (fresh block: no previous tables); every lane calls.  predef: the predefined table
+// of the same kind.  firstCode = code of sequence 0 (setRLE uses b.sequences[0]).  Normalisation, table fill and size
+// estimates use all lanes; the NCount is written by lane 0.
+// row: optional profiling stamps (stamp_clock) 0 start, 1 normalised, 2 table filled, 3 sizes estimated, 4 NCount written.
+B2C_DEV void seq_build_table(SeqTableWork *st, const FseCTable *predef, uint32_t symbolLen, uint32_t nseq,
+                             uint32_t firstCode, unsigned lane, unsigned long long *row) {
+    stamp_clock(row, 0);
+    FseCTable *ct = &st->cur;
+    const uint32_t *hist = st->hist;
     uint32_t maxCount = warp_max(hist[lane] > hist[lane + 32] ? hist[lane] : hist[lane + 32]);   // bins >= symbolLen are zero
+    const uint32_t tableLog = seq_optimal_tablelog(nseq, symbolLen);
     if (lane == 0) {
         ct->symbolLen = symbolLen;
-        ct->tableLog = seq_optimal_tablelog(nseq, symbolLen);
+        ct->tableLog = tableLog;
         ct->rleVal = 0;
     }
     if (maxCount == nseq) {
@@ -134,102 +130,39 @@ B2C_DEV void seq_build_table(SeqWork *sw, int which, uint32_t nseq, uint32_t fir
         if (lane == 0) {
             ct->useRLE = 1; ct->rleVal = firstCode; ct->tableLog = 0;
             ct->stateTable[0] = 0; ct->deltaNbBits[firstCode] = 0; ct->deltaFindState[firstCode] = 0;
-            sw->mode[which] = 1; sw->used[which] = 1;
-            sw->ncount[which][0] = (uint8_t)firstCode; sw->ncountLen[which] = 1;
+            st->mode = 1; st->used = 1;
+            st->ncount[0] = (uint8_t)firstCode; st->ncountLen = 1;
         }
         __syncwarp();
         return;
     }
     ct->norm[lane] = 0; ct->norm[lane + 32] = 0;
+    if (lane == 0) ct->useRLE = 0;
     __syncwarp();
-    int bad = 0;
-    if (lane == 0) {
-        ct->useRLE = 0;
-        bad = fse_normalize(hist, symbolLen, nseq, ct->tableLog, ct->norm);
-    }
-    bad = __shfl_sync(FULLMASK, bad, 0);
-    __syncwarp();
-    if (!bad) bad = fse_build_ctable_warp(ct, sw->fseScratch[which], lane);
+    int bad = fse_normalize(hist, symbolLen, nseq, tableLog, ct->norm, lane);
+    stamp_clock(row, 1);
+    if (!bad) bad = fse_build_ctable_warp(ct, st->fseScratch, lane);
+    stamp_clock(row, 2);
     if (bad) {
-        if (lane == 0) { sw->mode[which] = 0; sw->used[which] = 0; sw->ncountLen[which] = SEQ_TABLE_ERR; }
+        if (lane == 0) { st->mode = 0; st->used = 0; st->ncountLen = SEQ_TABLE_ERR; }
         __syncwarp();
         return;
     }
+    // chooseComp, blockenc.go:633-661 (prev == never valid for an independent block)
+    uint32_t nSize = fse_approx_size(ct, hist, symbolLen, lane) + (((symbolLen * tableLog) >> 3) + 3) * 8;
+    const uint32_t predefSize = fse_approx_size(predef, hist, symbolLen, lane);
+    nSize = nSize + ((nSize + 2 * 8 * 16) >> 4);
+    stamp_clock(row, 3);
     if (lane == 0) {
-        // chooseComp, blockenc.go:633-661 (prev == never valid for an independent block)
-        uint32_t nSize = fse_approx_size(ct, hist, symbolLen) + (((symbolLen * ct->tableLog) >> 3) + 3) * 8;
-        uint32_t predefSize = fse_approx_size(&sw->predef[which], hist, symbolLen);
-        nSize = nSize + ((nSize + 2 * 8 * 16) >> 4);
-        if (predefSize <= nSize) { sw->mode[which] = 0; sw->used[which] = 0; sw->ncountLen[which] = 0; }
+        if (predefSize <= nSize) { st->mode = 0; st->used = 0; st->ncountLen = 0; }
         else {
-            sw->mode[which] = 2; sw->used[which] = 1;
-            int w = fse_write_ncount(ct->norm, symbolLen, ct->tableLog, sw->ncount[which]);
-            if (w < 0) { sw->mode[which] = 0; sw->used[which] = 0; sw->ncountLen[which] = SEQ_TABLE_ERR; }
-            else sw->ncountLen[which] = (uint32_t)w;
+            st->mode = 2; st->used = 1;
+            int w = fse_write_ncount(ct->norm, symbolLen, tableLog, st->ncount);
+            if (w < 0) { st->mode = 0; st->used = 0; st->ncountLen = SEQ_TABLE_ERR; }
+            else st->ncountLen = (uint32_t)w;
         }
+        stamp_clock(row, 4);
     }
-    __syncwarp();
-}
-
-B2C_DEV const FseCTable *seq_table(const SeqWork *sw, int which) {
-    return sw->used[which] ? &sw->cur[which] : &sw->predef[which];
-}
-
-// One warp walks chain `which` over t = 1..nseq-1 (t = 0 is the last sequence) and stores
-// stb[idx] = (state & mask(nb)) | nb << 12 for idx = nseq-1-t.  codes[] is indexed by sequence.
-B2C_DEV void seq_chain(SeqWork *sw, int which, const uint8_t *codes, uint32_t nseq, uint16_t *stb) {
-    const FseCTable *ct = seq_table(sw, which);
-    unsigned lane = lane_id();
-    uint32_t m = nseq - 1;  // number of steps
-    if (ct->useRLE) {
-        for (uint32_t t = 1 + lane; t <= m; t += 32) stb[nseq - 1 - t] = 0;
-        if (lane == 0) sw->finalState[which] = 0;
-        __syncwarp();
-        return;
-    }
-    uint32_t seg = (m + 31) / 32;
-    uint32_t t0 = 1 + lane * seg;
-    uint32_t t1 = t0 + seg;  // exclusive
-    if (t0 > m + 1) t0 = m + 1;
-    if (t1 > m + 1) t1 = m + 1;
-    // assumed start state (state after step t0-1)
-    uint32_t start;
-    {
-        uint32_t tw = (t0 > (uint32_t)SEQ_WARMUP) ? t0 - SEQ_WARMUP : 1;  // first warm-up step
-        uint32_t st = fse_init_state(ct, codes[nseq - 1 - (tw - 1)]);
-        for (uint32_t t = tw; t < t0; t++) {
-            uint32_t sym = codes[nseq - 1 - t];
-            uint32_t nb = (st + ct->deltaNbBits[sym]) >> 16;
-            st = ct->stateTable[(int32_t)(st >> nb) + (int32_t)ct->deltaFindState[sym]];
-        }
-        start = st;
-    }
-    bool need = true;   // segment must be (re)computed
-    uint32_t fin = start;
-    for (;;) {
-        if (need) {
-            uint32_t st = start;
-            for (uint32_t t = t0; t < t1; t++) {
-                uint32_t sym = codes[nseq - 1 - t];
-                uint32_t nb = (st + ct->deltaNbBits[sym]) >> 16;
-                stb[nseq - 1 - t] = (uint16_t)((st & ((1u << nb) - 1)) | (nb << 12));
-                st = ct->stateTable[(int32_t)(st >> nb) + (int32_t)ct->deltaFindState[sym]];
-            }
-            fin = st;
-            need = false;
-        }
-        // verify against the predecessor's final state; lane 0 is exact by construction
-        uint32_t prevFin = __shfl_up_sync(FULLMASK, fin, 1);
-        bool bad = (lane > 0) && (t0 <= m) && (prevFin != start);
-        unsigned badMask = __ballot_sync(FULLMASK, bad);
-        if (badMask == 0) break;
-        // only the lowest mismatching lane is guaranteed to see a verified predecessor
-        if (lane == (unsigned)(__ffs((int)badMask) - 1)) { start = prevFin; need = true; }
-    }
-    // final state = state after step m: held by the last lane that has work (or lane 0 when m == 0)
-    uint32_t lastLane = (m == 0) ? 0 : (m - 1) / seg;
-    uint32_t f = __shfl_sync(FULLMASK, fin, (int)lastLane);
-    if (lane == 0) sw->finalState[which] = f;
     __syncwarp();
 }
 

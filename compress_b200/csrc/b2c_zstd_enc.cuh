@@ -125,6 +125,11 @@ struct ZstdEncParams {
             P.dbg_cycles[((uint64_t)chunk * 16 + (k)) * 32 + 16 + (threadIdx.x >> 5)] = (unsigned long long)clock64(); \
     } while (0)
 #endif
+// The same stamps in K2 (tools/tables_phase_times.py), taken by lane 0 of the warp that builds the table (stamp_clock):
+// the Huffman build stamps row 12 of the chunk, the LL / OF / ML builds rows 13..15 (rows the parse does not use).
+B2C_DEV unsigned long long *tables_stamp_row(const ZstdEncParams &P, uint32_t chunk, int row) {
+    return P.dbg_cycles ? P.dbg_cycles + ((uint64_t)chunk * 16 + 12 + (uint32_t)row) * 32 : nullptr;
+}
 
 B2C_DEV uint32_t chunk_size(const ZstdEncParams &P, uint32_t c) {
     if (P.desc) return P.desc[c].len;
@@ -287,63 +292,91 @@ B2C_DEV uint32_t snappy_put_copy(uint8_t *d, uint32_t off, uint32_t len) {   // 
 }
 
 // ------------------------------------------------------------------------------------------------ K2
-// One 128-thread CTA per chunk.  Warp 0 builds the Huffman table cooperatively (rank sort with 32 lanes, the
-// serial tree / setMaxHeight / table serialisation on lane 0); lane 0 of warps 1..3 builds one FSE table each.
+// Every warp of a K2 CTA builds all four tables of its own chunks, one chunk after another: the Huffman table (rank
+// sort, depths, code values, weight normalisation and table fill by all 32 lanes; the tree merge, setMaxHeight's repair
+// and the weight encode on lane 0), then the LL, OF and ML tables (normalisation, table fill and size estimates by all
+// lanes; the NCount on lane 0).  The warps share only the predefined tables and never wait for each other, so an SM keeps
+// one table build in flight per resident warp.
 #ifndef TABLES_MIN_CTAS
-#define TABLES_MIN_CTAS 8      // resident K2 CTAs per SM the register allocation is held to
+#define TABLES_MIN_CTAS 5      // resident K2 CTAs per SM the register allocation is held to (44 KB shared memory each)
 #endif
 constexpr int TABLES_NT = 128;
-struct TablesShared {
+constexpr int TABLES_NW = TABLES_NT / 32;
+struct TablesWarp {
     HufWork hw;
-    SeqWork sw;
+    SeqTableWork st;
 };
-B2C_DEV void zstd_tables_chunk(TablesShared *ts, const ZstdEncParams &P, uint32_t chunk) {
-    const unsigned tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+struct TablesShared {
+    SeqWork sw;                 // the predefined tables
+    TablesWarp wk[TABLES_NW];
+};
+B2C_DEV void zstd_tables_chunk(const SeqWork *sw, TablesWarp *tw, const ZstdEncParams &P, uint32_t chunk) {
+    const unsigned lane = threadIdx.x & 31;
     ChunkWork *W = P.work + chunk;
     if (W->kind != 0) return;
     const uint32_t nseq = W->nseq, nlit = W->nlit;
-    if (w == 0) {
-        HufWork *hw = &ts->hw;
+    {
+        HufWork *hw = &tw->hw;
+        unsigned long long *hrow = tables_stamp_row(P, chunk, 0);
         for (uint32_t s = lane; s < 256; s += 32) hw->count[s] = W->litHist[s];
         if (lane == 0) { hw->status = HUF_INCOMPRESSIBLE; hw->tableDescLen = 0; hw->tableLog = 0; }
         __syncwarp();
-        if (nlit > 16) huf_build_table(hw, nlit, lane, 32, -1);
-        __syncwarp();
+        stamp_clock(hrow, 0);
+        if (nlit > 16) {
+            huf_bt_stats(hw, nlit, lane);
+            __syncwarp();
+            if (hw->status == HUF_OK) {
+                huf_bt_sort(hw, lane, 32);
+                __syncwarp();
+                stamp_clock(hrow, 1);
+                if (lane == 0) huf_bt_merge(hw);
+                __syncwarp();
+                stamp_clock(hrow, 2);
+                huf_bt_depths(hw, lane);
+                stamp_clock(hrow, 3);
+                huf_bt_ranks(hw, nlit, lane);
+                stamp_clock(hrow, 4);
+                huf_bt_bits(hw, lane, 32);
+                __syncwarp();
+                huf_bt_vals(hw, lane, 32);
+                __syncwarp();
+                stamp_clock(hrow, 5);
+                huf_bt_write(hw, lane);
+                stamp_clock(hrow, 6);
+            }
+        }
         if (hw->status == HUF_OK) {
             for (uint32_t s = lane; s < 256; s += 32) { W->ctVal[s] = hw->ctVal[s]; W->ctBits[s] = hw->ctBits[s]; }
             for (uint32_t i = lane; i < hw->tableDescLen; i += 32) W->tableDesc[i] = hw->tableDesc[i];
         }
         if (lane == 0) { W->hufStatus = (uint32_t)hw->status; W->hufTableLog = hw->tableLog; W->tableDescLen = hw->tableDescLen; }
-    } else {
-        const int which = (int)w - 1;
-        SeqWork *sw = &ts->sw;
-        for (uint32_t s = lane; s < 64; s += 32) sw->hist[which][s] = W->seqHist[which][s];
-        if (lane == 0) sw->maxSym[which] = W->maxSym[which];
+        stamp_clock(hrow, 7);
+    }
+    for (int which = 0; which < 3; which++) {
+        SeqTableWork *st = &tw->st;
+        unsigned long long *srow = tables_stamp_row(P, chunk, 1 + which);
+        for (uint32_t s = lane; s < 64; s += 32) st->hist[s] = W->seqHist[which][s];
         __syncwarp();
-        seq_build_table(sw, which, nseq, wk_codes(P, chunk, which)[0], lane);
-        __syncwarp();
+        seq_build_table(st, &sw->predef[which], W->maxSym[which] + 1, nseq, wk_codes(P, chunk, which)[0], lane, srow);
         // publish the table this chain will use
-        const FseCTable *t = seq_table(sw, which);
+        const FseCTable *t = st->used ? &st->cur : &sw->predef[which];
         const uint32_t *s32 = reinterpret_cast<const uint32_t *>(t);
         uint32_t *d32 = reinterpret_cast<uint32_t *>(&W->tbl[which]);
         for (uint32_t i = lane; i < sizeof(FseCTable) / 4; i += 32) d32[i] = s32[i];
-        for (uint32_t i = lane; i < sw->ncountLen[which] && i < 96; i += 32) W->ncount[which][i] = sw->ncount[which][i];
+        for (uint32_t i = lane; i < st->ncountLen && i < 96; i += 32) W->ncount[which][i] = st->ncount[i];
         if (lane == 0) {
-            W->mode[which] = sw->mode[which]; W->ncountLen[which] = sw->ncountLen[which];
-            if (sw->ncountLen[which] == SEQ_TABLE_ERR) { W->ncountLen[which] = 0; W->kind = 1; }  // internal error: store raw
+            W->mode[which] = st->mode; W->ncountLen[which] = st->ncountLen;
+            if (st->ncountLen == SEQ_TABLE_ERR) { W->ncountLen[which] = 0; W->kind = 1; }  // internal error: store raw
         }
+        __syncwarp();
+        stamp_clock(srow, 5);
     }
 }
 
-// The chunk loop of a K2 CTA (chunks first, first + stride, ...).  K2 is bound by instruction issue, not by latency:
-// its serial stretches run with one active lane, and at 8 CTAs per SM the schedulers are about half busy.  Splitting
-// the Huffman work over two warps (codes / table description, pipelined over consecutive chunks) was measured and
-// changed nothing; what helps is fewer warp instructions (e.g. the sort over 2^ceil(log2(symbolLen)) keys).
+// The chunk loop of a K2 CTA: warp w takes chunks first * TABLES_NW + w, then every stride * TABLES_NW-th one.
 B2C_DEV void zstd_tables_loop(TablesShared *ts, const ZstdEncParams &P, uint32_t first, uint32_t stride) {
-    for (uint32_t c = first; c < P.nchunks; c += stride) {
-        zstd_tables_chunk(ts, P, c);
-        __syncthreads();
-    }
+    const unsigned w = threadIdx.x >> 5;
+    for (uint32_t c = first * TABLES_NW + w; c < P.nchunks; c += stride * TABLES_NW) zstd_tables_chunk(&ts->sw, &ts->wk[w], P, c);
 }
 
 // ------------------------------------------------------------------------------------------------ K3
