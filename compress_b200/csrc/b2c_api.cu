@@ -539,7 +539,7 @@ static int launch_encode(b2c_ctx *ctx, int level, int flags, const void *d_src, 
                 b2c_lz_parse3_kernel<<<g1, LzCfg<5>::NT, LzLayout<5>::SMEM_BYTES, st>>>(P);
             }
             PEV(2);
-            const unsigned gh = sms * 7 < m ? sms * 7 : m;
+            const unsigned gh = sms * HIST_CTAS_PER_SM < m ? sms * HIST_CTAS_PER_SM : m;
             b2c_zstd_hist_kernel<<<gh, HIST_NT, HIST_SMEM_BYTES, st>>>(P);
             ctx->launches += 2;
         }

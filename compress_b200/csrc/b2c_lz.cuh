@@ -1025,54 +1025,55 @@ B2C_DEV void lz_parse_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chun
 }
 
 // ------------------------------------------------------------------------------------------------ histograms
-// One 128-thread CTA per chunk: literal histogram (one private u8 counter per (symbol, lane) and warp -- no atomics, no
-// races; literals are counted in slices small enough that a counter cannot wrap) and the three sequence-code
-// histograms (ballot counts, lane l owns the codes whose low 5 bits equal l) with their highest used code.  Input:
-// the literals and codes the parse kernel left in the work pool.  (Round 1 did this inside the parse kernel, where it
-// pinned 64 KiB of shared memory; as a separate kernel it runs at seven CTAs per SM.)
+// One 128-thread CTA per chunk counts the literals and the three sequence-code streams the parse kernel left in the work
+// pool, in one pass over all four: the chunk's 16-byte pieces (literals first, then the LL, OF and ML codes) are dealt
+// round-robin to the threads, and every thread has the loads of HIST_BATCH pieces in flight before it counts the first.
+// The 448 bins (256 literal bytes, then 64 codes per table) are u32 shared-memory counters kept in HIST_COPIES copies,
+// lane l adding into copy l % 16 with shared-memory atomics: two lanes of a warp at most meet on one word or one bank.
+// Zeroing and reducing the copies is 28 KB of shared memory per chunk, independent of the chunk's size; the counting is
+// one atomic per byte.  Outputs: litHist, seqHist and the highest used code of each table (maxSym).  Seven CTAs share an
+// SM (28 KB of shared memory each).
 constexpr int HIST_NT = 128;
-constexpr int HIST_WARPS = HIST_NT / 32;
-constexpr uint32_t HIST_SLICE = 15u * 16u * HIST_NT; // bytes per slice: a lane takes 16-byte pieces, at most 15 of them (240 <= 255)
-constexpr uint32_t HIST_SMEM_BYTES = HIST_WARPS * 256 * 32;
-// Private-counter byte histogram of stream[s0, s1) (s0 a multiple of 16, stream 16-byte aligned): every lane owns one
-// byte counter per symbol (col[sym * 32]), reads 16 bytes per step with the next step's load already in flight, and merges
-// equal symbols inside a word so that the four updates of a word are independent.  At most 255 symbols per lane and call.
-template <uint32_t SYMMASK>
-B2C_DEV void hist_count_stream(const uint8_t *stream, uint32_t s0, uint32_t s1, uint8_t *col, unsigned tid) {
-    const uint4 *s16 = reinterpret_cast<const uint4 *>(stream);
-    const uint32_t n16 = (s1 + 15) / 16;
-    uint32_t i = s0 / 16 + tid;
-    uint4 v = (i < n16) ? B2C_LDG(s16 + i) : make_uint4(0, 0, 0, 0);
-    while (i < n16) {
-        const uint32_t inext = i + HIST_NT;
-        const uint4 vnext = (inext < n16) ? B2C_LDG(s16 + inext) : make_uint4(0, 0, 0, 0);   // requested before this one is used
-        const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const uint32_t pos = 16 * i + 4 * k;
-            if (pos < s1) {
-                const uint32_t nv = (pos + 4 <= s1) ? 4u : s1 - pos;
-                const uint32_t x = wv[k];
-                const uint32_t a0 = x & SYMMASK, a1 = (x >> 8) & SYMMASK, a2 = (x >> 16) & SYMMASK, a3 = (x >> 24) & SYMMASK;
-                uint32_t i0 = 1, i1 = nv > 1, i2 = nv > 2, i3 = nv > 3;
-                if (a1 == a0) { i0 += i1; i1 = 0; }
-                if (a2 == a0) { i0 += i2; i2 = 0; } else if (a2 == a1) { i1 += i2; i2 = 0; }
-                if (a3 == a0) { i0 += i3; i3 = 0; } else if (a3 == a1) { i1 += i3; i3 = 0; } else if (a3 == a2) { i2 += i3; i3 = 0; }
-                const uint32_t c0 = col[a0 * 32], c1 = col[a1 * 32], c2 = col[a2 * 32], c3 = col[a3 * 32];
-                col[a0 * 32] = (uint8_t)(c0 + i0);
-                if (i1) col[a1 * 32] = (uint8_t)(c1 + i1);
-                if (i2) col[a2 * 32] = (uint8_t)(c2 + i2);
-                if (i3) col[a3 * 32] = (uint8_t)(c3 + i3);
-            }
-        }
-        i = inext; v = vnext;
+constexpr int HIST_CTAS_PER_SM = 7;
+constexpr uint32_t HIST_BINS = 256 + 3 * 64;
+constexpr uint32_t HIST_COPIES = 16;
+constexpr uint32_t HIST_BATCH = 8;                 // 16-byte loads in flight per thread
+constexpr uint32_t HIST_CNT_WORDS = HIST_BINS * HIST_COPIES;
+constexpr uint32_t HIST_SMEM_BYTES = HIST_CNT_WORDS * 4 + 8 * 4;   // counters, then the six code-ballot words
+static_assert(HIST_COPIES == 16, "the reduction reads a bin's copies as four 16-byte quarters");
+
+// Piece p of a chunk's four streams: literal pieces [0, nl16), then nc16 pieces of each code stream (stride maxseq, a
+// multiple of 16).  len: bytes of the piece that belong to the stream; bin0 / mask: where its bytes are counted.
+struct HistPiece {
+    const uint8_t *src;
+    uint32_t len, bin0, mask;
+};
+B2C_DEV HistPiece hist_piece(const uint8_t *lit, const uint8_t *codes, uint32_t mseq, uint32_t nlit, uint32_t nseq,
+                             uint32_t nl16, uint32_t nc16, uint32_t p) {
+    HistPiece h;
+    if (p < nl16) {
+        h.src = lit + 16 * p; h.len = nlit - 16 * p; h.bin0 = 0; h.mask = 255;
+    } else {
+        const uint32_t q = p - nl16, c = (q >= nc16) + (q >= 2 * nc16), j = q - c * nc16;
+        h.src = codes + c * mseq + 16 * j; h.len = nseq - 16 * j; h.bin0 = 256 + 64 * c; h.mask = 63;
     }
+    if (h.len > 16) h.len = 16;
+    return h;
+}
+
+// Counts the four bytes of x into this lane's counters (lcnt: the lane's copy of the stream's first bin): one atomic per
+// byte, adding 0 for the bytes from nv on (past the end of the stream).  No merge of equal bytes: the compare-and-select
+// chain costs more than the atomics it saves.
+B2C_DEV void hist_count_word(uint32_t *lcnt, uint32_t x, uint32_t nv) {
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) atomicAdd(lcnt + ((x >> (8 * k)) & 0xffu) * HIST_COPIES, k < nv ? 1u : 0u);
 }
 
 B2C_DEV void zstd_hist_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chunk) {
-    const unsigned tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    const unsigned tid = threadIdx.x, lane = tid & 31;
     ChunkWork *W = P.work + chunk;
     const uint32_t nlit = W->nlit, nseq = W->nseq;
+    B2C_HIST_PHASE(0);
     const uint8_t *lit = wk_lit(P, chunk);
     if (P.dbg_hdr && W->kind != 3) {
         const WkLens wlen = wk_lens(P, chunk);
@@ -1085,76 +1086,73 @@ B2C_DEV void zstd_hist_chunk(uint8_t *smem, const ZstdEncParams &P, uint32_t chu
             for (uint32_t i = tid; i < nlit; i += HIST_NT) P.dbg_lits[(uint64_t)chunk * P.blockmax + i] = lit[i];
     }
     if (W->kind != 0) return;
-    uint32_t acc0 = 0, acc1 = 0;                       // symbols tid and tid + 128
-    uint8_t *hcol = smem + w * 256 * 32 + lane;
-    for (uint32_t s0 = 0; s0 < nlit; s0 += HIST_SLICE) {
-        const uint32_t s1 = (s0 + HIST_SLICE < nlit) ? s0 + HIST_SLICE : nlit;
-        for (uint32_t i = tid; i < HIST_SMEM_BYTES / 4; i += HIST_NT) reinterpret_cast<uint32_t *>(smem)[i] = 0;
-        __syncthreads();
-        hist_count_stream<255>(lit, s0, s1, hcol, tid);
-        __syncthreads();
-#pragma unroll
-        for (int half = 0; half < 2; half++) {
-            const uint32_t sym = tid + 128 * half;
-            uint32_t c = 0;
-#pragma unroll
-            for (int k = 0; k < HIST_WARPS; k++) {
-                const uint32_t *row = reinterpret_cast<const uint32_t *>(smem + k * 256 * 32 + sym * 32);
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    const uint32_t v = row[(j + (tid >> 2)) & 7];     // rotated: the 32 threads of a warp spread over the banks
-                    c += (v & 0xff) + ((v >> 8) & 0xff) + ((v >> 16) & 0xff) + (v >> 24);
-                }
-            }
-            if (half == 0) acc0 += c; else acc1 += c;
-        }
-        __syncthreads();
-    }
-    W->litHist[tid] = acc0;
-    W->litHist[tid + 128] = acc1;
-    // sequence-code counts: the same private byte counters, one 64-row table per code stream and warp
-    uint32_t cacc = 0, acc1c = 0;                       // code bins tid and tid + 128 (bin = table * 64 + code)
+    uint32_t *cnt = reinterpret_cast<uint32_t *>(smem);
+    uint32_t *nzw = cnt + HIST_CNT_WORDS;
+    // (the previous chunk's last reads of the counters are behind its final barrier)
+    for (uint32_t i = tid; i < HIST_CNT_WORDS / 4; i += HIST_NT) reinterpret_cast<uint4 *>(cnt)[i] = make_uint4(0, 0, 0, 0);
+    __syncthreads();
+    B2C_HIST_PHASE(1);
     const uint8_t *codes = wk_codes(P, chunk, 0);
-    const uint32_t mseq = P.maxseq;
-    for (uint32_t s0 = 0; s0 < nseq; s0 += HIST_SLICE) {
-        const uint32_t s1 = (s0 + HIST_SLICE < nseq) ? s0 + HIST_SLICE : nseq;
-        for (uint32_t i = tid; i < HIST_SMEM_BYTES / 4; i += HIST_NT) reinterpret_cast<uint32_t *>(smem)[i] = 0;
-        __syncthreads();
+    const uint32_t mseq = P.maxseq, nl16 = (nlit + 15) / 16, nc16 = (nseq + 15) / 16, npieces = nl16 + 3 * nc16;
+    uint32_t *lcnt = cnt + lane % HIST_COPIES;
+    for (uint32_t p0 = tid; p0 < npieces; p0 += HIST_NT * HIST_BATCH) {
+        uint4 v[HIST_BATCH];
 #pragma unroll
-        for (int c = 0; c < 3; c++) {
-            uint8_t *ccol = smem + w * 256 * 32 + c * 64 * 32 + lane;
-            hist_count_stream<63>(codes + (uint32_t)c * mseq, s0, s1, ccol, tid);      // maxseq is a multiple of 16
+        for (uint32_t k = 0; k < HIST_BATCH; k++) {
+            const uint32_t p = p0 + k * HIST_NT;
+            v[k] = p < npieces ? B2C_LDG(reinterpret_cast<const uint4 *>(hist_piece(lit, codes, mseq, nlit, nseq, nl16, nc16, p).src))
+                               : make_uint4(0, 0, 0, 0);
         }
-        __syncthreads();
-        for (uint32_t i = tid; i < 192; i += HIST_NT) {     // (HIST_NT = 128: two rounds; the accumulator is per (round, thread))
-            uint32_t c = 0;
 #pragma unroll
-            for (int k = 0; k < HIST_WARPS; k++) {
-                const uint32_t *row = reinterpret_cast<const uint32_t *>(smem + k * 256 * 32 + i * 32);
+        for (uint32_t k = 0; k < HIST_BATCH; k++) {
+            const uint32_t p = p0 + k * HIST_NT;
+            if (p < npieces) {
+                const HistPiece h = hist_piece(lit, codes, mseq, nlit, nseq, nl16, nc16, p);
+                const uint32_t m4 = h.mask * 0x01010101u;
+                const uint32_t wv[4] = {v[k].x & m4, v[k].y & m4, v[k].z & m4, v[k].w & m4};
+                uint32_t *bcnt = lcnt + h.bin0 * HIST_COPIES;
+                if (h.len == 16) {
 #pragma unroll
-                for (int jj = 0; jj < 8; jj++) {
-                    const uint32_t v = row[(jj + (tid >> 2)) & 7];
-                    c += (v & 0xff) + ((v >> 8) & 0xff) + ((v >> 16) & 0xff) + (v >> 24);
+                    for (uint32_t q = 0; q < 4; q++) hist_count_word(bcnt, wv[q], 4);
+                } else {                                      // the last piece of a stream
+#pragma unroll
+                    for (uint32_t q = 0; q < 4; q++) hist_count_word(bcnt, wv[q], h.len > 4 * q ? h.len - 4 * q : 0u);
                 }
             }
-            if (i < HIST_NT) cacc += c; else acc1c += c;
         }
-        __syncthreads();
-    }
-    uint32_t *shist = reinterpret_cast<uint32_t *>(smem);      // 6 ballot words
-    for (uint32_t i = tid; i < 192; i += HIST_NT) {
-        const uint32_t c = (i < HIST_NT) ? cacc : acc1c;
-        W->seqHist[i / 64][i % 64] = c;
-        // highest used code of each table: index groups of 32 are warp-aligned
-        const unsigned nz = __ballot_sync(FULLMASK, c != 0);
-        if ((i & 31) == 0) shist[i >> 5] = nz;
     }
     __syncthreads();
+    B2C_HIST_PHASE(2);
+    // thread t sums the copies of bins t + 128 k; a bin's four 16-byte quarters are read in an order rotated by t / 2, so
+    // the eight threads of one 16-byte load phase touch distinct banks
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        const uint32_t b = tid + k * HIST_NT;
+        if (b < HIST_BINS) {                                  // (k = 3: warps 0 and 1 only)
+            const uint4 *row = reinterpret_cast<const uint4 *>(cnt + b * HIST_COPIES);
+            uint32_t c = 0;
+#pragma unroll
+            for (uint32_t q = 0; q < 4; q++) {
+                const uint4 x = row[(q + (tid >> 1)) & 3];
+                c += x.x + x.y + x.z + x.w;
+            }
+            if (k < 2) {
+                W->litHist[b] = c;
+            } else {
+                const uint32_t s = b - 256;
+                W->seqHist[s >> 6][s & 63] = c;
+                // highest used code of each table: the 32 bins of a warp are 32 consecutive codes of one table
+                const unsigned nz = __ballot_sync(FULLMASK, c != 0);
+                if (lane == 0) nzw[s >> 5] = nz;
+            }
+        }
+    }
+    __syncthreads();
+    B2C_HIST_PHASE(3);
     if (tid < 3) {
-        const uint32_t lo = shist[2 * tid], hi = shist[2 * tid + 1];
+        const uint32_t lo = nzw[2 * tid], hi = nzw[2 * tid + 1];
         W->maxSym[tid] = hi ? 32 + (31 - (uint32_t)__clz((int)hi)) : (lo ? 31 - (uint32_t)__clz((int)lo) : 0u);
     }
-    __syncthreads();
 }
 
 #ifndef B2C_EMU
@@ -1189,7 +1187,7 @@ B2C_LZ_KERNEL(b2c_lz_snappy_better_kernel, 4, LZ_MODE_SNAPPY)
 B2C_LZ_KERNEL(b2c_lz_s2_best_kernel, LZ_S2BEST, LZ_MODE_S2)
 B2C_LZ_KERNEL(b2c_lz_snappy_best_kernel, LZ_S2BEST, LZ_MODE_SNAPPY)
 #undef B2C_LZ_KERNEL
-extern "C" __global__ void __launch_bounds__(HIST_NT) b2c_zstd_hist_kernel(ZstdEncParams P) {
+extern "C" __global__ void __launch_bounds__(HIST_NT, HIST_CTAS_PER_SM) b2c_zstd_hist_kernel(ZstdEncParams P) {
     extern __shared__ __align__(1024) uint8_t smem[];
     for (uint32_t c = blockIdx.x; c < P.nchunks; c += gridDim.x) zstd_hist_chunk(smem, P, c);
 }

@@ -125,6 +125,17 @@ struct ZstdEncParams {
             P.dbg_cycles[((uint64_t)chunk * 16 + (k)) * 32 + 16 + (threadIdx.x >> 5)] = (unsigned long long)clock64(); \
     } while (0)
 #endif
+// The same stamps in the hist kernel (tools/hist_phase_times.py): warp w takes row 12 + w, columns 8..15 (beside the
+// tables kernel's columns 0..7 of those rows).
+#ifdef B2C_EMU
+#define B2C_HIST_PHASE(k) do { } while (0)
+#else
+#define B2C_HIST_PHASE(k)                                                                              \
+    do {                                                                                               \
+        if (P.dbg_cycles && (threadIdx.x & 31) == 0)                                                   \
+            P.dbg_cycles[((uint64_t)chunk * 16 + 12 + (threadIdx.x >> 5)) * 32 + 8 + (k)] = (unsigned long long)clock64(); \
+    } while (0)
+#endif
 // The same stamps in K2 (tools/tables_phase_times.py), taken by lane 0 of the warp that builds the table (stamp_clock):
 // the Huffman build stamps row 12 of the chunk, the LL / OF / ML builds rows 13..15 (rows the parse does not use).
 B2C_DEV unsigned long long *tables_stamp_row(const ZstdEncParams &P, uint32_t chunk, int row) {
