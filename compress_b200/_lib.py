@@ -120,6 +120,13 @@ def _load():
     lib.b2c_s2_convert_lz4_chunks.restype = c.c_int
     lib.b2c_s2_convert_lz4_chunks.argtypes = [
         c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t]
+    lib.b2c_flate_decode_device.restype = c.c_int
+    lib.b2c_flate_decode_device.argtypes = [
+        c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p,
+        c.c_uint32, c.c_void_p, c.c_uint32, c.c_void_p]
+    lib.b2c_flate_decode_chunks.restype = c.c_int
+    lib.b2c_flate_decode_chunks.argtypes = [
+        c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t]
     lib.b2c_huf_compress_device.restype = c.c_int
     lib.b2c_huf_compress_device.argtypes = [
         c.c_void_p, c.c_int, c.c_void_p, c.c_size_t, c.c_void_p, c.c_uint32, c.c_void_p, c.c_size_t, c.c_void_p,
@@ -164,6 +171,7 @@ EXPORTED_SYMBOLS = [
     "b2c_zstd_frame_bound", "b2c_zstd_encode_frames_device", "b2c_zstd_encode_frames",
     "b2c_s2_stream_bound", "b2c_s2_encode_stream_device", "b2c_s2_encode_stream", "b2c_s2_decode_stream",
     "b2c_s2_convert_lz4_device", "b2c_s2_convert_lz4_chunks",
+    "b2c_flate_decode_device", "b2c_flate_decode_chunks",
 ]
 
 

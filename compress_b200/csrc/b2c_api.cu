@@ -22,6 +22,7 @@
 #include "b2c_s2_stream.cuh"
 #include "b2c_huf0.cuh"
 #include "b2c_lz4_cvt.cuh"
+#include "b2c_inflate.cuh"
 
 #ifndef TABLES_CTAS_PER_SM
 #define TABLES_CTAS_PER_SM TABLES_MIN_CTAS   // K2: resident CTAs per SM (44 KB static shared memory each)
@@ -87,6 +88,7 @@ struct b2c_ctx {
     Buf<> d_fr_io{kDevice, kExact};     // frame mode, host-buffer call: staged input | packed output | results
     Buf<> d_s2d{kDevice, kHeadroom};    // staged S2 block decode: block heads + element records
     Buf<> d_lzc{kDevice, kHeadroom};    // LZ4 -> S2 conversion: block heads + sequence records of one pass
+    Buf<> d_inf{kDevice, kHeadroom};    // inflate: input heads + match / stored-run / member records of one pass
     Buf<> d_s2best{kDevice, kExact};    // S2 best parse scratch (four candidates per position), reserved on first use
     Buf<> d_s2s{kDevice, kExact};       // S2 stream calls: block slots, sizes, checksums, scan, tables (grown on demand)
     Buf<> d_s2s_io{kDevice, kExact};    //   host-buffer calls: staged input | output
@@ -344,6 +346,7 @@ const char *b2c_strerror(int code) {
     case B2C_ERR_CRC: return "CRC check failed";
     case B2C_ERR_SIZE: return "frame size exceeded / mismatch";
     case B2C_ERR_UNSUPPORTED: return "unsupported";
+    case B2C_ERR_UNEXPECTED_EOF: return "unexpected end of input";
     default: return "unknown error";
     }
 }
@@ -1774,6 +1777,113 @@ int b2c_s2_convert_lz4_chunks(b2c_ctx *ctx, int format, int flags, const void *c
         if ((rc = scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st))) return rc;
     }
     return B2C_OK;
+}
+
+// ---- inflate: raw DEFLATE / zlib / gzip -------------------------------------------------------------------------
+// One pass decodes the inputs whose records fit kInfPassBytes of scratch (at least one input).  rec_base (device) holds
+// every input's first record when the host knows the sizes; otherwise every input gets room for max_src bytes into cap.
+static const uint64_t kInfPassBytes = (uint64_t)4 << 30;
+static int launch_inflate(b2c_ctx *ctx, InfParams P, uint32_t n, uint64_t max_src, uint64_t cap, const uint64_t *h_rec_base,
+                          cudaStream_t st) {
+    const uint64_t per = inf_rec_cap(max_src, cap);
+    { int r = ctx_order_begin(ctx, st); if (r) return r; }
+    for (uint32_t c0 = 0; c0 < n;) {
+        uint32_t c1 = c0 + 1;
+        uint64_t recs;
+        if (h_rec_base) {
+            while (c1 < n && (h_rec_base[c1 + 1] - h_rec_base[c0]) * sizeof(InfRec) <= kInfPassBytes) c1++;
+            recs = h_rec_base[c1] - h_rec_base[c0];
+        } else {
+            const uint64_t fit = kInfPassBytes / (per * sizeof(InfRec));
+            c1 = (uint32_t)((uint64_t)c0 + (fit > 1 ? fit : 1) < n ? c0 + (fit > 1 ? fit : 1) : n);
+            recs = (uint64_t)(c1 - c0) * per;
+        }
+        const uint32_t m = c1 - c0;
+        Layout L;
+        const size_t oHead = L.take((size_t)m * sizeof(InfHead)), oRec = L.take((size_t)recs * sizeof(InfRec));
+        { int r = reserve(ctx, ctx->d_inf, L.end); if (r) return r; }
+        P.c0 = c0; P.nchunks = m; P.rec_per = per;
+        P.heads = ctx->d_inf.at<InfHead>(oHead);
+        P.recs = ctx->d_inf.at<InfRec>(oRec);
+        b2c_inflate_walk_kernel<<<(m + INF_WALK_LANES - 1) / INF_WALK_LANES, INF_WALK_LANES, 0, st>>>(P);
+        b2c_inflate_exec_kernel<<<(m + INF_WARPS - 1) / INF_WARPS, INF_WARPS * 32, 0, st>>>(P);
+        b2c_inflate_check_kernel<<<(m + INF_WARPS - 1) / INF_WARPS, INF_WARPS * 32, 0, st>>>(P);
+        ctx->launches += 3;
+        CK(cudaGetLastError());
+        c0 = c1;
+    }
+    return ctx_order_end(ctx, st);
+}
+static bool flate_args_ok(int format, int flags) {
+    return (format == B2C_FLATE_RAW || format == B2C_FLATE_ZLIB || format == B2C_FLATE_GZIP) && !(flags & ~B2C_GZIP_SINGLE);
+}
+
+int b2c_flate_decode_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                            const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, void *d_dst, size_t dst_stride,
+                            const uint64_t *d_dst_offsets, uint32_t dst_cap, int64_t *d_out_sizes, uint32_t nchunks, void *stream) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if (!flate_args_ok(format, flags)) return B2C_ERR_ARG;
+    if (!d_src_sizes || !d_out_sizes || src_stride == 0 || src_stride > 0xffffffffull) return B2C_ERR_ARG;
+    if (nchunks == 0) return B2C_OK;
+    CK(cudaSetDevice(ctx->device));
+    InfParams P;
+    memset(&P, 0, sizeof(P));
+    P.src_base = (const uint8_t *)d_src; P.src_stride = src_stride; P.src_offsets = d_src_offsets; P.src_sizes = d_src_sizes;
+    P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_offsets = d_dst_offsets; P.dst_cap = dst_cap;
+    P.out_sizes = d_out_sizes;
+    P.format = format; P.multistream = !(flags & B2C_GZIP_SINGLE);
+    return launch_inflate(ctx, P, nchunks, src_stride, dst_cap, nullptr, (cudaStream_t)stream);
+}
+
+int b2c_flate_decode_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                            void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, size_t n) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if (!flate_args_ok(format, flags)) return B2C_ERR_ARG;
+    if (n == 0) return B2C_OK;
+    if (n > 0xffffffffull) return B2C_ERR_ARG;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    BatchMeta meta(n);
+    const BatchMeta::Arrays &h = meta.h;
+    std::vector<uint64_t> rec_base(n + 1);
+    uint64_t inb = 0, outb = 0, nrec = 0;
+    for (size_t i = 0; i < n; i++) {
+        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
+        h.src_off[i] = inb; h.dst_off[i] = outb;
+        h.src_sizes[i] = (uint32_t)src_sizes[i];
+        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
+        rec_base[i] = nrec;
+        nrec += inf_rec_cap(src_sizes[i], h.dst_caps[i]);
+        inb += (src_sizes[i] + 15) & ~(size_t)15;
+        outb += ((size_t)h.dst_caps[i] + 15) & ~(size_t)15;
+    }
+    rec_base[n] = nrec;
+    Layout L;
+    const size_t oMeta = L.take(meta.host.size()), oBase = L.take((n + 1) * sizeof(uint64_t));
+    std::vector<uint8_t> hostMeta(L.end);
+    memcpy(hostMeta.data() + oMeta, meta.host.data(), meta.host.size());
+    memcpy(hostMeta.data() + oBase, rec_base.data(), (n + 1) * sizeof(uint64_t));
+    int rc;
+    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_meta, L.end))) return rc;
+    if ((rc = gather_h2d(ctx, srcs, src_sizes, h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
+    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, hostMeta.data(), hostMeta.size(), cudaMemcpyHostToDevice, st));
+    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p + oMeta);
+    InfParams P;
+    memset(&P, 0, sizeof(P));
+    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
+    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
+    P.out_sizes = d.res;
+    P.rec_base = ctx->d_dec_meta.at<uint64_t>(oBase);
+    P.format = format; P.multistream = !(flags & B2C_GZIP_SINGLE);
+    if ((rc = launch_inflate(ctx, P, (uint32_t)n, 0, 0, rec_base.data(), st))) return rc;
+    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    std::vector<size_t> lens(n, 0);
+    for (size_t i = 0; i < n; i++)
+        if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
+    return scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st);
 }
 
 // ---- standalone huff0 blocks ------------------------------------------------------------------------

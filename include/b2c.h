@@ -41,7 +41,8 @@ enum {
     B2C_ERR_WINDOW = -8,        /* zstd.ErrWindowSizeExceeded / ErrWindowSizeTooSmall / ErrBlockTooBig-class */
     B2C_ERR_CRC = -9,           /* zstd.ErrCRCMismatch */
     B2C_ERR_SIZE = -10,         /* zstd.ErrFrameSizeExceeded / ErrFrameSizeMismatch / ErrDecoderSizeExceeded */
-    B2C_ERR_UNSUPPORTED = -11
+    B2C_ERR_UNSUPPORTED = -11,
+    B2C_ERR_UNEXPECTED_EOF = -12 /* inflate: io.ErrUnexpectedEOF (the input ends inside a stream, header or trailer) */
 };
 
 /* flags for the zstd encoder */
@@ -234,6 +235,37 @@ B2C_API int b2c_s2_convert_lz4_device(b2c_ctx *ctx, int format, int flags, const
 B2C_API int b2c_s2_convert_lz4_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
                                       void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, int64_t *decoded,
                                       size_t n);
+
+/*
+ * Inflate: raw DEFLATE, zlib and gzip streams (flate.NewReader, flate/inflate.go; zlib.NewReader, zlib/reader.go;
+ * gzip.NewReader, gzip/gunzip.go -- each read to the end).  Input i holds one stream of the given format: B2C_FLATE_RAW a
+ * DEFLATE stream (bytes after its final block are ignored), B2C_FLATE_ZLIB a zlib stream (Adler-32 checked; a preset
+ * dictionary is B2C_ERR_UNSUPPORTED unless it is the empty one; trailing bytes ignored), B2C_FLATE_GZIP one or more gzip
+ * members back to back (CRC-32 and ISIZE of each checked); with B2C_GZIP_SINGLE only the first member is read and the rest
+ * ignored (gzip.Reader.Multistream(false)).  Results: the content's bytes, or the reference's error class --
+ * B2C_ERR_CORRUPT (flate.CorruptInputError), B2C_ERR_UNEXPECTED_EOF (io.ErrUnexpectedEOF), B2C_ERR_MAGIC (gzip / zlib
+ * ErrHeader), B2C_ERR_CRC (ErrChecksum), B2C_ERR_UNSUPPORTED (zlib.ErrDictionary), B2C_ERR_DST_SMALL (the content does not
+ * fit dst_cap) -- the first in stream order; the reference's InternalError for a code-length symbol above 18 is
+ * B2C_ERR_CORRUPT.  A gzip input that ends before its first member's header is complete (an
+ * empty input included: gzip.NewReader returns io.EOF there) is B2C_ERR_UNEXPECTED_EOF.  As in the reference, a raw stream
+ * that ends inside the extra bits of a length or a distance yields the content decoded up to there.
+ * One lane decodes one stream (a stream is serial): throughput comes from batches of many inputs; a single long stream
+ * decodes at the speed of one lane.  Inputs and contents are under 4 GiB each.
+ * _device: argument conventions of b2c_s2_decode_device, asynchronous on `stream`.  Without d_src_offsets input i is at
+ * d_src + i * src_stride; with them src_stride is the bound on every input's size.  An input larger than src_stride is
+ * B2C_ERR_ARG.  Scratch for inf_rec_cap(src_stride, dst_cap) 16-byte records per input (about dst_cap / 3 + src_stride / 4)
+ * is held by the context; a call needing more than 4 GiB of it runs in passes, and the context keeps up to 5 GiB of device
+ * memory for them (4 GiB with 25 % headroom) -- 16 384 inputs into 64 KiB each already take two passes.
+ * _chunks: host buffers, synchronous.
+ */
+enum { B2C_FLATE_RAW = 0, B2C_FLATE_ZLIB = 1, B2C_FLATE_GZIP = 2 };
+enum { B2C_GZIP_SINGLE = 1 };          /* gzip.Reader.Multistream(false) */
+B2C_API int b2c_flate_decode_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                                    const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, void *d_dst,
+                                    size_t dst_stride, const uint64_t *d_dst_offsets, uint32_t dst_cap,
+                                    int64_t *d_out_sizes, uint32_t nchunks, void *stream);
+B2C_API int b2c_flate_decode_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                                    void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, size_t n);
 
 /*
  * S2 / Snappy STREAMS (the framing format: s2.Writer.EncodeBuffer, s2/writer.go:357-470, and s2.Reader over a buffer,
