@@ -23,6 +23,7 @@
 #include "b2c_huf0.cuh"
 #include "b2c_lz4_cvt.cuh"
 #include "b2c_inflate.cuh"
+#include "b2c_deflate.cuh"
 
 #ifndef TABLES_CTAS_PER_SM
 #define TABLES_CTAS_PER_SM TABLES_MIN_CTAS   // K2: resident CTAs per SM (44 KB static shared memory each)
@@ -89,6 +90,7 @@ struct b2c_ctx {
     Buf<> d_s2d{kDevice, kHeadroom};    // staged S2 block decode: block heads + element records
     Buf<> d_lzc{kDevice, kHeadroom};    // LZ4 -> S2 conversion: block heads + sequence records of one pass
     Buf<> d_inf{kDevice, kHeadroom};    // inflate: input heads + match / stored-run / member records of one pass
+    Buf<> d_dfl{kDevice, kHeadroom};    // stateless deflate: per-input writer state | gzip header | block slots of one pass
     Buf<> d_s2best{kDevice, kExact};    // S2 best parse scratch (four candidates per position), reserved on first use
     Buf<> d_s2s{kDevice, kExact};       // S2 stream calls: block slots, sizes, checksums, scan, tables (grown on demand)
     Buf<> d_s2s_io{kDevice, kExact};    //   host-buffer calls: staged input | output
@@ -1879,6 +1881,150 @@ int b2c_flate_decode_chunks(b2c_ctx *ctx, int format, int flags, const void *con
     P.format = format; P.multistream = !(flags & B2C_GZIP_SINGLE);
     if ((rc = launch_inflate(ctx, P, (uint32_t)n, 0, 0, rec_base.data(), st))) return rc;
     CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    std::vector<size_t> lens(n, 0);
+    for (size_t i = 0; i < n; i++)
+        if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
+    return scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st);
+}
+
+// ---- stateless deflate: flate.StatelessDeflate / gzip at StatelessCompression ---------------------------------------
+// Block slot g = input * max_blocks + k; one pass parses and encodes the slots [g0, g1), at most kDflPassSlots of them
+// (about 1 GiB of tokens).  Each input's bit writer lives in d_dfl, so an input whose blocks span passes continues.
+static const uint64_t kDflPassSlots = 8192;
+size_t b2c_flate_stateless_bound(size_t n, size_t dict_len) {
+    (void)dict_len;                                     // a dict only moves the first cut: at most one block more
+    return n + 8 * (n / DFL_STEP + 3) + 16;
+}
+static int launch_deflate(b2c_ctx *ctx, DflParams P, uint32_t n, const void *hdr, size_t hlen, cudaStream_t st) {
+    Layout L;
+    const size_t oState = L.take((size_t)n * sizeof(DflState)), oHdr = L.take(hlen ? hlen : 1);
+    const uint64_t total = (uint64_t)n * P.max_blocks;
+    const uint64_t per = total < kDflPassSlots ? total : kDflPassSlots;
+    const size_t oSlots = L.take((size_t)per * sizeof(DflSlot)), oTok = L.take((size_t)per * DFL_SLOT_TOKENS * 4);
+    { int r = reserve(ctx, ctx->d_dfl, L.end); if (r) return r; }
+    { int r = ctx_order_begin(ctx, st); if (r) return r; }
+    P.state = ctx->d_dfl.at<DflState>(oState);
+    P.slots = ctx->d_dfl.at<DflSlot>(oSlots);
+    P.tokens = ctx->d_dfl.at<uint32_t>(oTok);
+    P.hdr = ctx->d_dfl.p + oHdr; P.hlen = (uint32_t)hlen;
+    if (hlen) CK(cudaMemcpyAsync(ctx->d_dfl.p + oHdr, hdr, hlen, cudaMemcpyHostToDevice, st));
+    for (uint64_t g0 = 0; g0 < total; g0 += per) {
+        P.g0 = g0; P.g1 = g0 + per < total ? g0 + per : total;
+        const uint32_t i0 = (uint32_t)(P.g0 / P.max_blocks), i1 = (uint32_t)((P.g1 + P.max_blocks - 1) / P.max_blocks);
+        b2c_deflate_parse_kernel<<<(unsigned)((P.g1 - P.g0 + DFL_PARSE_WARPS - 1) / DFL_PARSE_WARPS), DFL_PARSE_WARPS * 32, 0, st>>>(P, n);
+        b2c_deflate_encode_kernel<<<(i1 - i0 + DFL_ENCODE_LANES - 1) / DFL_ENCODE_LANES, DFL_ENCODE_LANES, 0, st>>>(P, i0, i1);
+        ctx->launches += 2;
+        CK(cudaGetLastError());
+    }
+    b2c_deflate_crc_kernel<<<(n + DFL_CRC_WARPS - 1) / DFL_CRC_WARPS, DFL_CRC_WARPS * 32, 0, st>>>(P, n);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    return ctx_order_end(ctx, st);
+}
+static bool deflate_args_ok(int format, int flags, const void *hdr, size_t hlen) {
+    if (flags != 0 || (format != B2C_FLATE_RAW && format != B2C_FLATE_GZIP)) return false;
+    if (format == B2C_FLATE_GZIP) return hdr && hlen >= 10 && hlen < (1u << 20);
+    return hlen == 0;
+}
+
+int b2c_flate_stateless_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                               const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, const uint8_t *d_eof,
+                               const void *d_dict, const uint64_t *d_dict_offsets, const uint32_t *d_dict_sizes,
+                               const void *hdr, size_t hlen, void *d_dst, size_t dst_stride, const uint64_t *d_dst_offsets,
+                               uint32_t dst_cap, int64_t *d_out_sizes, const uint32_t *d_crc_in, uint32_t *d_crc_out,
+                               uint32_t nchunks, void *stream) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if (!deflate_args_ok(format, flags, hdr, hlen)) return B2C_ERR_ARG;
+    if (!d_src_sizes || !d_out_sizes || src_stride == 0 || src_stride > 0xffffffffull) return B2C_ERR_ARG;
+    if (d_dict_sizes && (!d_dict || !d_dict_offsets)) return B2C_ERR_ARG;
+    if (format == B2C_FLATE_GZIP && (d_dict_sizes || d_eof)) return B2C_ERR_ARG;       // a gzip member has neither
+    if (nchunks == 0) return B2C_OK;
+    CK(cudaSetDevice(ctx->device));
+    DflParams P;
+    memset(&P, 0, sizeof(P));
+    P.src_base = (const uint8_t *)d_src; P.src_stride = src_stride; P.src_offsets = d_src_offsets; P.src_sizes = d_src_sizes;
+    P.dict_base = (const uint8_t *)d_dict; P.dict_offsets = d_dict_offsets; P.dict_sizes = d_dict_sizes;
+    P.eof = d_eof;
+    P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_offsets = d_dst_offsets; P.dst_cap = dst_cap;
+    P.out_sizes = d_out_sizes; P.crc_in = d_crc_in; P.crc_out = d_crc_out;
+    P.format = format;
+    const uint32_t mb = dfl_blocks(src_stride, d_dict_sizes ? DFL_DICT : 0);
+    P.max_blocks = mb ? mb : 1;
+    return launch_deflate(ctx, P, nchunks, hdr, hlen, (cudaStream_t)stream);
+}
+
+int b2c_flate_stateless_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                               const uint8_t *eof, const void *const *dicts, const size_t *dict_sizes, const void *hdr,
+                               size_t hlen, void *const *dsts, const size_t *dst_caps, int64_t *sizes_out,
+                               const uint32_t *crc_in, uint32_t *crc_out, size_t n) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if (!deflate_args_ok(format, flags, hdr, hlen)) return B2C_ERR_ARG;
+    if (n == 0) return B2C_OK;
+    if (n > 0xffffffffull || (dicts != nullptr) != (dict_sizes != nullptr)) return B2C_ERR_ARG;
+    if (format == B2C_FLATE_GZIP && (dicts || eof)) return B2C_ERR_ARG;      // a gzip member has neither
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    BatchMeta meta(n);
+    const BatchMeta::Arrays &h = meta.h;
+    uint64_t inb = 0, outb = 0, db = 0;
+    uint32_t mb = 1;
+    std::vector<uint64_t> dict_off(n, 0);
+    std::vector<uint32_t> dict_sz(n, 0);
+    for (size_t i = 0; i < n; i++) {
+        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
+        h.src_off[i] = inb; h.dst_off[i] = outb;
+        h.src_sizes[i] = (uint32_t)src_sizes[i];
+        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
+        const size_t dl = dicts ? (dict_sizes[i] > DFL_DICT ? DFL_DICT : dict_sizes[i]) : 0;   // only the last 8 KiB count
+        dict_off[i] = db; dict_sz[i] = (uint32_t)dl;
+        const uint32_t b = dfl_blocks(src_sizes[i], (uint32_t)dl);
+        if (b > mb) mb = b;
+        inb += (src_sizes[i] + 15) & ~(size_t)15;
+        outb += ((size_t)h.dst_caps[i] + 15) & ~(size_t)15;
+        db += (dl + 15) & ~(size_t)15;
+    }
+    Layout L;
+    const size_t oMeta = L.take(meta.host.size()), oDo = L.take(n * 8), oDs = L.take(n * 4), oEof = L.take(n),
+                 oCrc = L.take(n * 4), oCrcOut = L.take(n * 4), oDict = L.take(db + 16);
+    std::vector<uint8_t> hostMeta(oDict);
+    memcpy(hostMeta.data() + oMeta, meta.host.data(), meta.host.size());
+    memcpy(hostMeta.data() + oDo, dict_off.data(), n * 8);
+    memcpy(hostMeta.data() + oDs, dict_sz.data(), n * 4);
+    for (size_t i = 0; i < n; i++) hostMeta[oEof + i] = eof ? eof[i] : 1;
+    if (crc_in) memcpy(hostMeta.data() + oCrc, crc_in, n * 4);
+    int rc;
+    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
+    if ((rc = reserve(ctx, ctx->d_dec_meta, L.end))) return rc;
+    if ((rc = gather_h2d(ctx, srcs, src_sizes, h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
+    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, hostMeta.data(), hostMeta.size(), cudaMemcpyHostToDevice, st));
+    if (dicts) {
+        std::vector<const void *> dp(n);
+        std::vector<size_t> dl(n);
+        for (size_t i = 0; i < n; i++) {
+            dl[i] = dict_sz[i];
+            dp[i] = dl[i] ? (const uint8_t *)dicts[i] + (dict_sizes[i] - dl[i]) : dicts[i];
+        }
+        if ((rc = gather_h2d(ctx, dp.data(), dl.data(), dict_off.data(), n, ctx->d_dec_meta.p + oDict, (size_t)db, st))) return rc;
+    }
+    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p + oMeta);
+    DflParams P;
+    memset(&P, 0, sizeof(P));
+    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
+    if (dicts) {
+        P.dict_base = ctx->d_dec_meta.p + oDict; P.dict_offsets = ctx->d_dec_meta.at<uint64_t>(oDo);
+        P.dict_sizes = ctx->d_dec_meta.at<uint32_t>(oDs);
+    }
+    P.eof = ctx->d_dec_meta.p + oEof;
+    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
+    P.out_sizes = d.res;
+    P.crc_in = crc_in ? ctx->d_dec_meta.at<uint32_t>(oCrc) : nullptr;
+    P.crc_out = ctx->d_dec_meta.at<uint32_t>(oCrcOut);
+    P.format = format; P.max_blocks = mb;
+    if ((rc = launch_deflate(ctx, P, (uint32_t)n, hdr, hlen, st))) return rc;
+    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (crc_out) CK(cudaMemcpyAsync(crc_out, P.crc_out, n * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     std::vector<size_t> lens(n, 0);
     for (size_t i = 0; i < n; i++)

@@ -1,6 +1,10 @@
 """Inflate on the device: raw DEFLATE, zlib and gzip streams in batches (the reader side of the reference's flate, zlib and
 gzip packages: flate/inflate.go, zlib/reader.go, gzip/gunzip.go).
 
+Encoder.encode_chunks / encode_device write flate.StatelessDeflate output (flate/stateless.go) for a batch of inputs, raw
+or as gzip members, byte-identical to the reference: every block of every input is parsed at once on the device.
+StatelessDeflate and NewStatelessWriter are thin layers over one such call.
+
 Decoder.decode_chunks / decode_device decode a batch of whole streams in one call, one lane per stream; results are the
 content's bytes or the reference's error class (B2C_ERR_* codes, see include/b2c.h).  NewReader and the readers of the gzip
 and zlib modules are thin layers over one such call for a single input: a single stream is serial, so one long stream
@@ -18,6 +22,9 @@ RAW, ZLIB, GZIP = 0, 1, 2                    # B2C_FLATE_RAW / _ZLIB / _GZIP
 GZIP_SINGLE = 1                              # B2C_GZIP_SINGLE: gzip.Reader.Multistream(false)
 ERR_DST_SMALL, ERR_CORRUPT, ERR_MAGIC, ERR_CRC, ERR_UNSUPPORTED, ERR_UNEXPECTED_EOF = -4, -5, -7, -9, -11, -12
 MAX_CAP = (1 << 32) - 1                      # contents are under 4 GiB
+
+
+MAX_STATELESS_DICT = 8 << 10                 # only the last 8 KiB of a dict are used
 
 
 class CorruptInputError(Exception):
@@ -136,3 +143,139 @@ def NewReader(r):
     (one GPU lane).  Returns an io.BytesIO of the content; errors are raised here."""
     data = r if isinstance(r, (bytes, bytearray, memoryview)) else r.read()
     return io.BytesIO(_decoder().decode_all(bytes(data), RAW))
+
+
+def StatelessBound(n, dict_len=0):
+    """The largest raw StatelessDeflate output of an n-byte input."""
+    return int(lib.b2c_flate_stateless_bound(n, dict_len))
+
+
+class Encoder:
+    """Batches of flate.StatelessDeflate calls (raw) or gzip members at StatelessCompression, encoded on one GPU."""
+
+    def __init__(self, device=0):
+        if lib.b2c_device_count() <= 0:
+            raise B2CError("no CUDA device")
+        self._ctx = lib.b2c_ctx_create(device, 0)
+        if not self._ctx:
+            raise B2CError("b2c_ctx_create failed")
+
+    def close(self):
+        if self._ctx:
+            lib.b2c_ctx_destroy(self._ctx)
+            self._ctx = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def encode_device(self, src, src_sizes, src_stride, dst=None, dst_cap=None, out_sizes=None, format=RAW, eof=None,
+                      dict=None, dict_offsets=None, dict_sizes=None, header=b"", crc_in=None, crc_out=None,
+                      src_offsets=None):
+        """Device-resident batch: input i is src_sizes[i] bytes at src + i * src_stride (or src + src_offsets[i]); its
+        output goes to row i of dst ([n, dst_cap] uint8).  eof: optional uint8 per input (raw only, default all true);
+        dict / dict_offsets / dict_sizes: optional per-input dicts (raw only); header: the gzip member header (format
+        GZIP); crc_in / crc_out: optional uint32 (int32 tensors) CRC-32 seeds and results.  Asynchronous on the current
+        stream.  Returns (dst, out_sizes): out_sizes[i] = bytes or a negative B2C_ERR_* code."""
+        assert src.is_cuda and src.dtype == torch.uint8
+        n = src_sizes.numel()
+        if dst_cap is None:
+            dst_cap = StatelessBound(src_stride, MAX_STATELESS_DICT) + len(header) + 10
+        if dst is None:
+            dst = torch.empty((n, dst_cap), dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty((n,), dtype=torch.int64, device=src.device)
+        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        stream = torch.cuda.current_stream(src.device).cuda_stream
+        check(lib.b2c_flate_stateless_device(self._ctx, format, 0, src.data_ptr(), src_stride, ptr(src_offsets),
+                                             src_sizes.data_ptr(), ptr(eof), ptr(dict), ptr(dict_offsets), ptr(dict_sizes),
+                                             bytes(header), len(header), dst.data_ptr(),
+                                             dst.shape[1] if dst.dim() == 2 else dst_cap, None, dst_cap,
+                                             out_sizes.data_ptr(), ptr(crc_in), ptr(crc_out), n,
+                                             ctypes.c_void_p(stream)), self._ctx)
+        return dst, out_sizes
+
+    def encode_chunks(self, inputs, format=RAW, eof=None, dicts=None, header=b"", caps=None, crc_in=None):
+        """Host buffers: one StatelessDeflate call (raw) or one gzip member per input.  Returns (outputs, codes, crcs):
+        outputs[i] the bytes (None on error), codes[i] their length or a negative B2C_ERR_* code, crcs[i] the CRC-32 of
+        input i continued from crc_in[i]."""
+        n = len(inputs)
+        if n == 0:
+            return [], [], []
+        if caps is None:
+            caps = [StatelessBound(len(b), MAX_STATELESS_DICT) + len(header) + 10 for b in inputs]
+        keep = []
+
+        def arr(bs):
+            a = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(1, dtype=np.uint8) for b in bs]
+            keep.append(a)
+            return (ctypes.c_void_p * n)(*[x.ctypes.data for x in a])
+        srcs = arr(inputs)
+        ssz = (ctypes.c_size_t * n)(*[len(b) for b in inputs])
+        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
+        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
+        dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
+        eofs = None if eof is None else (ctypes.c_uint8 * n)(*[1 if e else 0 for e in eof])
+        dp = dsz = None
+        if dicts is not None:
+            dl = [d or b"" for d in dicts]
+            dp = arr(dl)
+            dsz = (ctypes.c_size_t * n)(*[len(d) for d in dl])
+        cin = None if crc_in is None else (ctypes.c_uint32 * n)(*crc_in)
+        cout = (ctypes.c_uint32 * n)()
+        res = (ctypes.c_int64 * n)()
+        check(lib.b2c_flate_stateless_chunks(self._ctx, format, 0, srcs, ssz, eofs, dp, dsz, bytes(header), len(header),
+                                             dsts, dcap, res, cin, cout, n), self._ctx)
+        codes = [int(r) for r in res]
+        return ([outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes,
+                [int(c) for c in cout])
+
+
+_enc = None
+
+
+def _encoder():
+    global _enc
+    if _enc is None:
+        _enc = Encoder()
+    return _enc
+
+
+def StatelessDeflate(out, in_, eof, dict=None):
+    """flate.StatelessDeflate: writes the stateless encoding of in_ to out (a binary file-like object), encoded on the
+    device in one call.  Only the last 8 KiB of dict are used."""
+    outs, codes, _ = _encoder().encode_chunks([bytes(in_)], RAW, eof=[eof], dicts=None if dict is None else [bytes(dict)])
+    if codes[0] < 0:
+        raise B2CError(f"libb200comp error {codes[0]}: {lib.b2c_strerror(codes[0]).decode()}")
+    out.write(outs[0])
+
+
+class _StatelessWriter:
+    """flate.NewStatelessWriter (flate/stateless.go:20-55): every Write is one StatelessDeflate(p, false) call, Close
+    writes the final empty block."""
+
+    def __init__(self, dst):
+        self._dst, self._closed = dst, False
+
+    def Write(self, p):
+        StatelessDeflate(self._dst, p, False)
+        return len(p)
+
+    write = Write
+
+    def Close(self):
+        if self._closed:
+            return
+        self._closed = True
+        StatelessDeflate(self._dst, b"", True)
+
+    close = Close
+
+    def Reset(self, w):
+        self._dst, self._closed = w, False
+
+
+def NewStatelessWriter(dst):
+    return _StatelessWriter(dst)

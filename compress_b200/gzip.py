@@ -1,11 +1,19 @@
 """gzip.NewReader on the device (gzip/gunzip.go): the members are decoded in one device call, on one GPU lane (a single
-input is serial; see flate.Decoder for batches).  The first member's Header is parsed on the host."""
+input is serial; see flate.Decoder for batches).  The first member's Header is parsed on the host.
+
+gzip.NewWriterLevel(w, StatelessCompression) (gzip/gzip.go): a Writer whose every Write is one device call of
+flate.StatelessDeflate; the CRC-32 is continued on the device.  Other levels are not built."""
 import io
 import struct
 from dataclasses import dataclass
 
 from . import flate
 from .flate import ErrUnexpectedEOF  # noqa: F401
+
+
+StatelessCompression = -3
+# time.Time{}.Unix(): the reference writes uint32(ModTime.Unix()) without a zero check, so an unset ModTime is this
+ZERO_MODTIME = -62135596800
 
 
 class ErrHeader(Exception):
@@ -88,3 +96,71 @@ class Reader:
 def NewReader(r):
     """gzip.NewReader: a Reader over r (bytes-like or a binary file)."""
     return Reader(r)
+
+
+class Writer:
+    """gzip.Writer at StatelessCompression: Name / Comment / Extra / ModTime (Unix seconds; unset is Go's zero time) / OS
+    set before the first
+    Write go into the header; each Write(p) is StatelessDeflate(p, false), Close writes StatelessDeflate(nil, true), the
+    CRC-32 and ISIZE.  Flush writes nothing (the stateless writer keeps no pending data)."""
+
+    def __init__(self, w, level=StatelessCompression):
+        if level != StatelessCompression:
+            raise ValueError("gzip: only StatelessCompression (-3) is built on the device; level %r is not" % (level,))
+        self.Reset(w)
+
+    def Reset(self, w):
+        """As the reference's Reset (gzip/gzip.go:98-114): the header fields go back to their zero values too."""
+        self.Name, self.Comment, self.Extra, self.ModTime, self.OS = "", "", None, ZERO_MODTIME, 255
+        self._w, self._wrote, self._closed, self._crc, self._size = w, False, False, 0, 0
+
+    def _header(self):
+        flg = (4 if self.Extra is not None else 0) | (8 if self.Name else 0) | (16 if self.Comment else 0)
+        h = b"\x1f\x8b\x08" + bytes([flg]) + struct.pack("<I", int(self.ModTime) & 0xffffffff) + b"\x00" + bytes([self.OS])
+        if self.Extra is not None:
+            h += struct.pack("<H", len(self.Extra)) + bytes(self.Extra)
+        if self.Name:
+            h += self.Name.encode("latin-1") + b"\x00"
+        if self.Comment:
+            h += self.Comment.encode("latin-1") + b"\x00"
+        return h
+
+    def Write(self, p):
+        p = bytes(p)
+        if not self._wrote:
+            self._wrote = True
+            self._w.write(self._header())
+        outs, codes, crcs = flate._encoder().encode_chunks([p], flate.RAW, eof=[False], crc_in=[self._crc])
+        if codes[0] < 0:
+            flate.raise_for(codes[0], flate.RAW)
+        self._w.write(outs[0])
+        self._crc = crcs[0]
+        self._size = (self._size + len(p)) & 0xffffffff
+        return len(p)
+
+    write = Write
+
+    def Flush(self):
+        pass
+
+    def Close(self):
+        if self._closed:
+            return
+        self._closed = True
+        if not self._wrote:
+            self.Write(b"")
+        self._w.write(b"\x03\x00" + struct.pack("<II", self._crc, self._size))
+
+    close = Close
+
+
+def NewWriterLevel(w, level):
+    """gzip.NewWriterLevel; only StatelessCompression is built."""
+    return Writer(w, level)
+
+
+def header_bytes(Name="", Comment="", Extra=None, ModTime=ZERO_MODTIME, OS=255):
+    """The member header gzip.Writer writes for these fields (XFL 0), as flate.Encoder takes it for format GZIP."""
+    w = Writer(io.BytesIO())
+    w.Name, w.Comment, w.Extra, w.ModTime, w.OS = Name, Comment, Extra, ModTime, OS
+    return w._header()

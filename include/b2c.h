@@ -268,6 +268,33 @@ B2C_API int b2c_flate_decode_chunks(b2c_ctx *ctx, int format, int flags, const v
                                     void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, size_t n);
 
 /*
+ * Stateless DEFLATE (flate.StatelessDeflate, flate/stateless.go:76-162), byte-identical to the reference on amd64.
+ * B2C_FLATE_RAW: input i is one StatelessDeflate(out, in, eof[i], dict_i) call (d_eof null: every eof is true).  Its output
+ * is byte-aligned and stands alone; with eof false it ends with an empty non-final stored block.  The optional dict of an
+ * input (d_dict_sizes null: none) counts with its last 8 KiB only.  B2C_FLATE_GZIP: input i is one gzip member as
+ * gzip.NewWriterLevel(w, StatelessCompression) writes it for one Write(p) then Close() (gzip/gzip.go:171-290): hdr (the
+ * member header, >= 10 bytes, built by the caller and copied into every member), StatelessDeflate(p, false),
+ * StatelessDeflate(nil, true), CRC-32 and ISIZE; eof and dicts do not apply (given, the call is B2C_ERR_ARG).  zlib has no stateless level.
+ * Results: the output's bytes, or B2C_ERR_DST_SMALL (nothing is written past the destination), or B2C_ERR_ARG for an
+ * input of the _device call larger than src_stride.  d_crc_out (optional)
+ * receives each input's CRC-32 continued from d_crc_in (optional seeds; the gzip trailer uses the continued value).
+ * Every block of every input is parsed at once (one warp per block); the bit writer then walks each input's blocks in
+ * order on one lane.  Inputs are under 4 GiB.  b2c_flate_stateless_bound(n, dict_len): the largest raw output of an
+ * n-byte input (add hlen + 10 for a gzip member).  Argument conventions as b2c_flate_decode_device / _chunks; flags is 0.
+ */
+B2C_API size_t b2c_flate_stateless_bound(size_t n, size_t dict_len);
+B2C_API int b2c_flate_stateless_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                                       const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, const uint8_t *d_eof,
+                                       const void *d_dict, const uint64_t *d_dict_offsets, const uint32_t *d_dict_sizes,
+                                       const void *hdr, size_t hlen, void *d_dst, size_t dst_stride,
+                                       const uint64_t *d_dst_offsets, uint32_t dst_cap, int64_t *d_out_sizes,
+                                       const uint32_t *d_crc_in, uint32_t *d_crc_out, uint32_t nchunks, void *stream);
+B2C_API int b2c_flate_stateless_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                                       const uint8_t *eof, const void *const *dicts, const size_t *dict_sizes,
+                                       const void *hdr, size_t hlen, void *const *dsts, const size_t *dst_caps,
+                                       int64_t *sizes_out, const uint32_t *crc_in, uint32_t *crc_out, size_t n);
+
+/*
  * S2 / Snappy STREAMS (the framing format: s2.Writer.EncodeBuffer, s2/writer.go:357-470, and s2.Reader over a buffer,
  * s2/reader.go:249-420; constants and the masked CRC32-C: s2/s2.go:75-126).  A stream = the identifier chunk, then per
  * block (<= 64 KiB here, WriterBlockSize) one chunk: type (0 compressed, 1 uncompressed), 24-bit length, checksum of the
