@@ -7,6 +7,9 @@ infrastructure and is never imported from here.
 import ctypes
 import os
 
+import numpy as np
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B2C_LIB") or os.path.join(_HERE, "_lib", "libb200comp.so")   # B2C_LIB: tuning builds
 
@@ -193,3 +196,61 @@ def check(rc, ctx=None):
         if ctx:
             msg += ": " + lib.b2c_last_cuda_error(ctx).decode()
         raise B2CError(f"libb200comp error {rc}: {msg}")
+
+
+class Context:
+    """Owner of one library context (b2c_ctx) on a CUDA device, freed by close(), at the end of a with block or with the
+    object.  Raises B2CError without a device: there is no CPU fallback."""
+
+    _ctx = None
+
+    def __init__(self, device=0, max_chunks=0):
+        if not torch.cuda.is_available() or lib.b2c_device_count() == 0:
+            raise B2CError("no CUDA device: compress_b200 has no CPU fallback")
+        self._ctx = lib.b2c_ctx_create(device, max_chunks)
+        if not self._ctx:
+            raise B2CError("b2c_ctx_create failed")
+
+    def close(self):
+        if self._ctx:
+            lib.b2c_ctx_destroy(self._ctx)
+            self._ctx = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
+class PointerTable:
+    """The arguments of a pointer-table call for n blobs: srcs / ssz (their addresses and sizes), dsts / dcap (one output
+    buffer of caps[i] bytes each) and res (the per-blob results), kept alive with the table.  An empty blob is passed as a
+    one-byte placeholder."""
+
+    def __init__(self, blobs, caps):
+        self.n = len(blobs)
+        self._keep = []
+        self.srcs = self.pointers(blobs)
+        self.ssz = (ctypes.c_size_t * self.n)(*[len(b) for b in blobs])
+        self.outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
+        self.dsts = (ctypes.c_void_p * self.n)(*[o.ctypes.data for o in self.outs])
+        self.dcap = (ctypes.c_size_t * self.n)(*[int(c) for c in caps])
+        self.res = (ctypes.c_int64 * self.n)()
+
+    def pointers(self, blobs):
+        """A c_void_p array of the blobs' addresses; the blobs' buffers live as long as the table."""
+        a = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(1, dtype=np.uint8) for b in blobs]
+        self._keep.append(a)
+        return (ctypes.c_void_p * len(a))(*[x.ctypes.data for x in a])
+
+    def results(self):
+        """-> (outputs, codes): outputs[i] the result's bytes, None where codes[i] is a negative error."""
+        codes = [int(r) for r in self.res]
+        return [o[:c].tobytes() if c >= 0 else None for o, c in zip(self.outs, codes)], codes

@@ -1027,25 +1027,119 @@ static int scatter_d2h(b2c_ctx *ctx, void *const *dsts, const size_t *lens, cons
     return B2C_OK;
 }
 
-// Per-item arrays of the zstd and S2 host-buffer batches: filled on the host, copied to the device in one piece.
-struct BatchMeta {
+}  // extern "C": HostBatch has member templates
+
+static uint32_t clamp32(size_t v) { return (uint32_t)(v > 0xffffffffull ? 0xffffffffull : v); }
+
+// One pointer-table batch: n caller pieces, their inputs placed in d_dec_in and their outputs in d_dec_out, and m device
+// items whose per-item arrays -- with the extra arrays a call lists -- form one layout that crosses to d_dec_meta in one
+// copy.  m == n except in zstd decode, whose items are frames.  Use: check(), place() / place_items(), stage_in(), the
+// launch, results(), scatter().
+struct HostBatch {
     struct Arrays { uint64_t *src_off, *dst_off; int64_t *res; uint32_t *src_sizes, *dst_caps; };
+    b2c_ctx *ctx;
+    size_t n, m;
+    std::vector<uint64_t> in_off, out_off;      // piece i's offset in d_dec_in / d_dec_out
+    uint64_t in_bytes = 0, out_bytes = 0;
+    Layout L;
     size_t off[5];
-    std::vector<uint8_t> host;
-    Arrays h;                                    // in `host`
-    explicit BatchMeta(size_t m) {
-        Layout L;
+    std::vector<size_t> ex;                     // offsets of the extra arrays, in the order given
+    std::vector<uint8_t> host;                  // the arrays and the extras; regions L takes later are device-only
+    Arrays h, d = {};                           // in `host` / in d_dec_meta (set by stage_in)
+
+    HostBatch(b2c_ctx *c, size_t n_, size_t m_, std::initializer_list<size_t> extra = {})
+        : ctx(c), n(n_), m(m_), in_off(n_), out_off(n_) {
         off[0] = L.take(sizeof(uint64_t) * m); off[1] = L.take(sizeof(uint64_t) * m); off[2] = L.take(sizeof(int64_t) * m);
         off[3] = L.take(sizeof(uint32_t) * m); off[4] = L.take(sizeof(uint32_t) * m);
+        for (size_t b : extra) ex.push_back(L.take(b));
         host.resize(L.end);
         h = at(host.data());
+    }
+    // The checks every pointer-table call makes after its own: the item count, then each input against the call's limit.
+    static int check(b2c_ctx *ctx, size_t n, const size_t *src_sizes, size_t limit) {
+        if (n > 0xffffffffull) return B2C_ERR_ARG;
+        CK(cudaSetDevice(ctx->device));
+        for (size_t i = 0; i < n; i++)
+            if (src_sizes[i] > limit) return B2C_ERR_ARG;
+        return B2C_OK;
     }
     Arrays at(uint8_t *base) const {
         return {reinterpret_cast<uint64_t *>(base + off[0]), reinterpret_cast<uint64_t *>(base + off[1]),
                 reinterpret_cast<int64_t *>(base + off[2]), reinterpret_cast<uint32_t *>(base + off[3]),
                 reinterpret_cast<uint32_t *>(base + off[4])};
     }
+    template <class T> T *h_at(size_t o) { return reinterpret_cast<T *>(host.data() + o); }
+    template <class T> T *d_at(size_t o) const { return ctx->d_dec_meta.at<T>(o); }
+    // Piece i's input and output offsets: packed at 16-byte alignment (stride 0) or at a fixed stride.
+    void place(const size_t *in_len, size_t in_stride, const size_t *out_len, size_t out_stride) {
+        for (size_t i = 0; i < n; i++) {
+            in_off[i] = in_bytes; out_off[i] = out_bytes;
+            in_bytes += in_stride ? in_stride : (in_len[i] + 15) & ~(uint64_t)15;
+            out_bytes += out_stride ? out_stride : ((uint64_t)clamp32(out_len[i]) + 15) & ~(uint64_t)15;
+        }
+    }
+    // place() with one item per piece: its input, its output and its capacity clamped to 32 bits.
+    void place_items(const size_t *src_sizes, size_t in_stride, const size_t *dst_caps, size_t out_stride) {
+        place(src_sizes, in_stride, dst_caps, out_stride);
+        for (size_t i = 0; i < n; i++) {
+            h.src_off[i] = in_off[i]; h.dst_off[i] = out_off[i];
+            h.src_sizes[i] = (uint32_t)src_sizes[i]; h.dst_caps[i] = clamp32(dst_caps[i]);
+        }
+    }
+    // Reserves the three buffers, gathers lens[i] bytes of srcs[i] into d_dec_in and uploads the arrays.
+    int stage_in(const void *const *srcs, const size_t *lens) {
+        int rc;
+        if ((rc = reserve(ctx, ctx->d_dec_in, in_bytes + 256))) return rc;
+        if ((rc = reserve(ctx, ctx->d_dec_out, out_bytes + 256))) return rc;
+        if ((rc = reserve(ctx, ctx->d_dec_meta, L.end + 256))) return rc;
+        if ((rc = gather_h2d(ctx, srcs, lens, in_off.data(), n, ctx->d_dec_in.p, in_bytes, ctx->stream))) return rc;
+        CK(cudaMemcpyAsync(ctx->d_dec_meta.p, host.data(), host.size(), cudaMemcpyHostToDevice, ctx->stream));
+        d = at(ctx->d_dec_meta.p);
+        return B2C_OK;
+    }
+    // A Params struct of a packed call with the batch's buffers and arrays; the rest zeroed.
+    template <class P> P params() const {
+        P p;
+        memset(&p, 0, sizeof(p));
+        p.src_base = ctx->d_dec_in.p; p.src_offsets = d.src_off; p.src_sizes = d.src_sizes;
+        p.dst_base = ctx->d_dec_out.p; p.dst_offsets = d.dst_off; p.dst_caps = d.dst_caps; p.out_sizes = d.res;
+        return p;
+    }
+    // The m results -> res (host), then synchronises: copies the call enqueued before complete with it.
+    int results(int64_t *res) {
+        CK(cudaMemcpyAsync(res, d.res, m * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        return B2C_OK;
+    }
+    // A result larger than its piece's capacity becomes B2C_ERR_DST_SMALL; then each positive result's bytes (or, with
+    // row, `row` bytes for each result >= 0) go to dsts[i].  Synchronises.
+    int scatter(void *const *dsts, int64_t *sizes, const size_t *dst_caps, size_t row = 0) {
+        std::vector<size_t> lens(n, 0);
+        for (size_t i = 0; i < n; i++) {
+            if (sizes[i] > 0 && (size_t)sizes[i] > dst_caps[i]) sizes[i] = B2C_ERR_DST_SMALL;
+            if (sizes[i] >= 0) lens[i] = row ? row : (size_t)sizes[i];
+        }
+        return scatter_d2h(ctx, dsts, lens.data(), out_off.data(), n, ctx->d_dec_out.p, out_bytes, ctx->stream);
+    }
 };
+
+// Record-bounded launches (LZ4 conversion, inflate): the pass that starts at item c0 takes the items whose records fit
+// kRecPassBytes of scratch, at least one.  rec_base (host) holds every item's first record, and the total at [n]; without it
+// every item has room for `per` records.  Sets *c1 to the pass's end and returns its record count.
+static const uint64_t kRecPassBytes = (uint64_t)4 << 30;
+static uint64_t next_pass(uint32_t c0, uint32_t n, const uint64_t *rec_base, uint64_t per, size_t rec_bytes, uint32_t *c1) {
+    if (rec_base) {
+        uint32_t e = c0 + 1;
+        while (e < n && (rec_base[e + 1] - rec_base[c0]) * rec_bytes <= kRecPassBytes) e++;
+        *c1 = e;
+        return rec_base[e] - rec_base[c0];
+    }
+    const uint64_t fit = kRecPassBytes / (per * rec_bytes), k = fit > 1 ? fit : 1;
+    *c1 = (uint32_t)((uint64_t)c0 + k < n ? c0 + k : n);
+    return (uint64_t)(*c1 - c0) * per;
+}
+
+extern "C" {
 
 // lit_span: bytes of the output layout (literal areas mirror it: input c's area starts at c * lit_stride, or at
 // dst_offsets[c] when lit_stride is 0 -- the caller then guarantees non-overlapping, increasing offsets); 0 = unknown: the
@@ -1215,21 +1309,18 @@ int b2c_zstd_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *
                            const size_t *dst_caps, int64_t *sizes_out, size_t n) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
     if (n == 0) return B2C_OK;
-    if (n > 0xffffffffull) return B2C_ERR_ARG;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
+    if (rc) return rc;
     // work items: one per frame (split inputs) or one per input (everything else)
     struct Item { size_t input; size_t src_off_in_input; uint32_t src_len; uint64_t dst_off_in_input; uint32_t cap; };
     std::vector<Item> items;
     std::vector<size_t> first_item(n + 1, 0);
-    std::vector<uint64_t> in_base(n), out_base(n), out_len(n);
+    std::vector<size_t> out_len(n);
     std::vector<char> split(n, 0);
-    uint64_t inb = 0, outb = 0;
     std::vector<FrameSpan> fr;
     for (size_t i = 0; i < n; i++) {
-        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
         first_item[i] = items.size();
-        const uint64_t cap = dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i];
+        const uint64_t cap = clamp32(dst_caps[i]);
         fr.clear();
         bool ok = src_sizes[i] > 0 && scan_frames((const uint8_t *)srcs[i], src_sizes[i], fr) && !fr.empty();
         uint64_t total = 0;
@@ -1239,7 +1330,6 @@ int b2c_zstd_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *
                 total += f.skippable ? 0 : f.fcs;
             }
         if (ok && total > cap) ok = false;               // the serial path reports the reference's "too large" error
-        in_base[i] = inb; out_base[i] = outb;
         if (ok) {
             split[i] = 1;
             uint64_t o = 0;
@@ -1253,34 +1343,23 @@ int b2c_zstd_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *
             items.push_back({i, 0, (uint32_t)src_sizes[i], 0, (uint32_t)cap});
             out_len[i] = cap;
         }
-        inb += (src_sizes[i] + 15) & ~(size_t)15;
-        outb += (out_len[i] + 15) & ~(uint64_t)15;
     }
     first_item[n] = items.size();
     const size_t m = items.size();
     if (m > 0xffffffffull) return B2C_ERR_ARG;
-    BatchMeta meta(m);
+    HostBatch B(ctx, n, m);
+    B.place(src_sizes, 0, out_len.data(), 0);
     for (size_t k = 0; k < m; k++) {
-        meta.h.src_off[k] = in_base[items[k].input] + items[k].src_off_in_input;
-        meta.h.dst_off[k] = out_base[items[k].input] + items[k].dst_off_in_input;
-        meta.h.src_sizes[k] = items[k].src_len; meta.h.dst_caps[k] = items[k].cap;
+        B.h.src_off[k] = B.in_off[items[k].input] + items[k].src_off_in_input;
+        B.h.dst_off[k] = B.out_off[items[k].input] + items[k].dst_off_in_input;
+        B.h.src_sizes[k] = items[k].src_len; B.h.dst_caps[k] = items[k].cap;
     }
-    int rc;
-    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 64))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 64))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_meta, meta.host.size()))) return rc;
-    if ((rc = gather_h2d(ctx, srcs, src_sizes, in_base.data(), n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, meta.host.data(), meta.host.size(), cudaMemcpyHostToDevice, st));
-    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p);
-    ZstdDecParams P;
-    memset(&P, 0, sizeof(P));
-    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
-    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
-    P.out_sizes = d.res; P.nchunks = (uint32_t)m;
-    if ((rc = launch_decode(ctx, P, st, outb, 0))) return rc;
+    if ((rc = B.stage_in(srcs, src_sizes))) return rc;
+    ZstdDecParams P = B.params<ZstdDecParams>();
+    P.nchunks = (uint32_t)m;
+    if ((rc = launch_decode(ctx, P, ctx->stream, B.out_bytes, 0))) return rc;
     std::vector<int64_t> res(m);
-    CK(cudaMemcpyAsync(res.data(), P.out_sizes, m * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    if ((rc = B.results(res.data()))) return rc;
     for (size_t i = 0; i < n; i++) {
         int64_t total = 0;
         for (size_t k = first_item[i]; k < first_item[i + 1]; k++) {
@@ -1294,14 +1373,8 @@ int b2c_zstd_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *
             total += res[k];
         }
         sizes_out[i] = total;
-        out_len[i] = total > 0 ? (uint64_t)total : 0;
     }
-    {
-        std::vector<size_t> lens(n);
-        for (size_t i = 0; i < n; i++) lens[i] = (size_t)out_len[i];
-        if ((rc = scatter_d2h(ctx, dsts, lens.data(), out_base.data(), n, ctx->d_dec_out.p, (size_t)outb, st))) return rc;
-    }
-    return B2C_OK;
+    return B.scatter(dsts, sizes_out, dst_caps);
 }
 
 
@@ -1606,58 +1679,25 @@ static int s2_host_batch(b2c_ctx *ctx, bool encode, int level, int flags, const 
                          void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, size_t n) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
     if (n == 0) return B2C_OK;
-    if (n > 0xffffffffull) return B2C_ERR_ARG;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    BatchMeta meta(n);
-    const BatchMeta::Arrays &h = meta.h;
-    uint64_t inb = 0, outb = 0;
-    for (size_t i = 0; i < n; i++) {
-        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
-        h.src_off[i] = inb; h.dst_off[i] = outb;
-        h.src_sizes[i] = (uint32_t)src_sizes[i];
-        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
-        // encode: fixed strides (the kernel addresses chunks by stride)
-        inb += encode ? (size_t)ENC_MAX_CHUNK : ((src_sizes[i] + 15) & ~(size_t)15);
-        outb += encode ? (size_t)kSlot : (((size_t)h.dst_caps[i] + 15) & ~(size_t)15);
-    }
-    int rc;
-    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_meta, meta.host.size()))) return rc;
-    {
-        std::vector<size_t> lens(n);
-        for (size_t i = 0; i < n; i++) {
-            lens[i] = src_sizes[i];
-            if (encode && src_sizes[i] > ENC_MAX_CHUNK) { h.src_sizes[i] = ENC_MAX_CHUNK + 1; lens[i] = 0; }   // reported as too big
-        }
-        if ((rc = gather_h2d(ctx, srcs, lens.data(), h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
-    }
-    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, meta.host.data(), meta.host.size(), cudaMemcpyHostToDevice, st));
-    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p);
-    if (encode)
-        rc = b2c_s2_encode_device(ctx, level, flags, ctx->d_dec_in.p, ENC_MAX_CHUNK, d.src_sizes, 0, ctx->d_dec_out.p, kSlot, d.res,
-                                  (uint32_t)n, st);
-    else {
-        S2DecParams P;
-        memset(&P, 0, sizeof(P));
-        P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
-        P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
-        P.out_sizes = d.res; P.nchunks = (uint32_t)n;
-        rc = launch_s2_decode(ctx, P, inb, st);
-    }
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    {
-        std::vector<size_t> lens(n, 0);
-        for (size_t i = 0; i < n; i++) {
-            if (sizes_out[i] > 0 && (size_t)sizes_out[i] > dst_caps[i]) { sizes_out[i] = B2C_ERR_DST_SMALL; continue; }
-            if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
-        }
-        if ((rc = scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st))) return rc;
+    HostBatch B(ctx, n, n);
+    // encode: fixed strides (the kernel addresses chunks by stride)
+    B.place_items(src_sizes, encode ? ENC_MAX_CHUNK : 0, dst_caps, encode ? kSlot : 0);
+    std::vector<size_t> lens(src_sizes, src_sizes + n);
+    for (size_t i = 0; i < n; i++)
+        if (encode && src_sizes[i] > ENC_MAX_CHUNK) { B.h.src_sizes[i] = ENC_MAX_CHUNK + 1; lens[i] = 0; }   // reported as too big
+    if ((rc = B.stage_in(srcs, lens.data()))) return rc;
+    if (encode)
+        rc = b2c_s2_encode_device(ctx, level, flags, ctx->d_dec_in.p, ENC_MAX_CHUNK, B.d.src_sizes, 0, ctx->d_dec_out.p, kSlot,
+                                  B.d.res, (uint32_t)n, ctx->stream);
+    else {
+        S2DecParams P = B.params<S2DecParams>();
+        P.nchunks = (uint32_t)n;
+        rc = launch_s2_decode(ctx, P, B.in_bytes, ctx->stream);
     }
-    return B2C_OK;
+    if (rc || (rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps);
 }
 
 int b2c_s2_encode_chunks(b2c_ctx *ctx, int level, int flags, const void *const *srcs, const size_t *src_sizes,
@@ -1672,24 +1712,14 @@ int b2c_s2_decode_chunks(b2c_ctx *ctx, const void *const *srcs, const size_t *sr
 
 
 // ---- LZ4 / LZ4s -> S2 / Snappy block conversion ---------------------------------------------------------
-// One pass converts the blocks whose records fit kLzcPassBytes of scratch (at least one block).  rec_base (device) holds
-// every block's first record when the host knows the sizes; otherwise every block gets room for a block of max_src bytes.
-static const uint64_t kLzcPassBytes = (uint64_t)4 << 30;
+// Passes of next_pass(); rec_base (device) holds every block's first record when the host knows the sizes, otherwise every
+// block gets room for a block of max_src bytes.
 static int launch_lz4_convert(b2c_ctx *ctx, LzcParams P, uint32_t n, uint64_t max_src, const uint64_t *h_rec_base,
                               cudaStream_t st) {
     const uint64_t per = (P.lz4s ? max_src / 2 : max_src / 3) + 1;
     { int r = ctx_order_begin(ctx, st); if (r) return r; }
-    for (uint32_t c0 = 0; c0 < n;) {
-        uint32_t c1 = c0 + 1;
-        uint64_t recs;
-        if (h_rec_base) {
-            while (c1 < n && (h_rec_base[c1 + 1] - h_rec_base[c0]) * sizeof(LzcRec) <= kLzcPassBytes) c1++;
-            recs = h_rec_base[c1] - h_rec_base[c0];
-        } else {
-            const uint64_t fit = kLzcPassBytes / (per * sizeof(LzcRec));
-            c1 = (uint32_t)((uint64_t)c0 + (fit > 1 ? fit : 1) < n ? c0 + (fit > 1 ? fit : 1) : n);
-            recs = (uint64_t)(c1 - c0) * per;
-        }
+    for (uint32_t c0 = 0, c1; c0 < n; c0 = c1) {
+        const uint64_t recs = next_pass(c0, n, h_rec_base, per, sizeof(LzcRec), &c1);
         const uint32_t m = c1 - c0;
         Layout L;
         const size_t oHead = L.take((size_t)m * sizeof(LzcHead)), oRec = L.take((size_t)recs * sizeof(LzcRec));
@@ -1701,7 +1731,6 @@ static int launch_lz4_convert(b2c_ctx *ctx, LzcParams P, uint32_t n, uint64_t ma
         b2c_lz4_cvt_emit_kernel<<<(m + LZC_EMIT_WARPS - 1) / LZC_EMIT_WARPS, LZC_EMIT_WARPS * 32, 0, st>>>(P);
         ctx->launches += 2;
         CK(cudaGetLastError());
-        c0 = c1;
     }
     return ctx_order_end(ctx, st);
 }
@@ -1729,77 +1758,35 @@ int b2c_s2_convert_lz4_chunks(b2c_ctx *ctx, int format, int flags, const void *c
     if (!ctx) return B2C_ERR_NO_DEVICE;
     if ((format != B2C_LZ4 && format != B2C_LZ4S) || (flags & ~B2C_S2_SNAPPY)) return B2C_ERR_ARG;
     if (n == 0) return B2C_OK;
-    if (n > 0xffffffffull) return B2C_ERR_ARG;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
+    if (rc) return rc;
     const bool lz4s = format == B2C_LZ4S;
-    BatchMeta meta(n);
-    const BatchMeta::Arrays &h = meta.h;
-    std::vector<uint64_t> rec_base(n + 1);
-    uint64_t inb = 0, outb = 0, nrec = 0;
-    for (size_t i = 0; i < n; i++) {
-        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
-        h.src_off[i] = inb; h.dst_off[i] = outb;
-        h.src_sizes[i] = (uint32_t)src_sizes[i];
-        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
-        rec_base[i] = nrec;
-        nrec += (lz4s ? src_sizes[i] / 2 : src_sizes[i] / 3) + 1;
-        inb += (src_sizes[i] + 15) & ~(size_t)15;
-        outb += ((size_t)h.dst_caps[i] + 15) & ~(size_t)15;
-    }
-    rec_base[n] = nrec;
-    // device metadata: the batch's arrays, then the record bases and the decoded lengths
-    Layout L;
-    const size_t oMeta = L.take(meta.host.size()), oBase = L.take((n + 1) * sizeof(uint64_t)), oDec = L.take(n * sizeof(int64_t));
-    std::vector<uint8_t> hostMeta(oDec);
-    memcpy(hostMeta.data() + oMeta, meta.host.data(), meta.host.size());
-    memcpy(hostMeta.data() + oBase, rec_base.data(), (n + 1) * sizeof(uint64_t));
-    int rc;
-    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_meta, L.end))) return rc;
-    if ((rc = gather_h2d(ctx, srcs, src_sizes, h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, hostMeta.data(), hostMeta.size(), cudaMemcpyHostToDevice, st));
-    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p + oMeta);
-    LzcParams P;
-    memset(&P, 0, sizeof(P));
-    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
-    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
-    P.out_sizes = d.res; P.decoded = ctx->d_dec_meta.at<int64_t>(oDec);
-    P.rec_base = ctx->d_dec_meta.at<uint64_t>(oBase);
+    HostBatch B(ctx, n, n, {(n + 1) * sizeof(uint64_t)});            // + the record bases
+    const size_t oDec = B.L.take(n * sizeof(int64_t));               // decoded lengths (device only)
+    B.place_items(src_sizes, 0, dst_caps, 0);
+    uint64_t *rec_base = B.h_at<uint64_t>(B.ex[0]);
+    rec_base[0] = 0;
+    for (size_t i = 0; i < n; i++) rec_base[i + 1] = rec_base[i] + (lz4s ? src_sizes[i] / 2 : src_sizes[i] / 3) + 1;
+    if ((rc = B.stage_in(srcs, src_sizes))) return rc;
+    LzcParams P = B.params<LzcParams>();
+    P.decoded = B.d_at<int64_t>(oDec);
+    P.rec_base = B.d_at<uint64_t>(B.ex[0]);
     P.lz4s = lz4s; P.snappy = (flags & B2C_S2_SNAPPY) != 0;
-    if ((rc = launch_lz4_convert(ctx, P, (uint32_t)n, 0, rec_base.data(), st))) return rc;
-    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(decoded_out, P.decoded, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    {
-        std::vector<size_t> lens(n, 0);
-        for (size_t i = 0; i < n; i++)
-            if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
-        if ((rc = scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st))) return rc;
-    }
-    return B2C_OK;
+    if ((rc = launch_lz4_convert(ctx, P, (uint32_t)n, 0, rec_base, ctx->stream))) return rc;
+    CK(cudaMemcpyAsync(decoded_out, P.decoded, n * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps);
 }
 
 // ---- inflate: raw DEFLATE / zlib / gzip -------------------------------------------------------------------------
-// One pass decodes the inputs whose records fit kInfPassBytes of scratch (at least one input).  rec_base (device) holds
-// every input's first record when the host knows the sizes; otherwise every input gets room for max_src bytes into cap.
-static const uint64_t kInfPassBytes = (uint64_t)4 << 30;
+// Passes of next_pass(); rec_base (device) holds every input's first record when the host knows the sizes, otherwise every
+// input gets room for max_src bytes into cap.
 static int launch_inflate(b2c_ctx *ctx, InfParams P, uint32_t n, uint64_t max_src, uint64_t cap, const uint64_t *h_rec_base,
                           cudaStream_t st) {
     const uint64_t per = inf_rec_cap(max_src, cap);
     { int r = ctx_order_begin(ctx, st); if (r) return r; }
-    for (uint32_t c0 = 0; c0 < n;) {
-        uint32_t c1 = c0 + 1;
-        uint64_t recs;
-        if (h_rec_base) {
-            while (c1 < n && (h_rec_base[c1 + 1] - h_rec_base[c0]) * sizeof(InfRec) <= kInfPassBytes) c1++;
-            recs = h_rec_base[c1] - h_rec_base[c0];
-        } else {
-            const uint64_t fit = kInfPassBytes / (per * sizeof(InfRec));
-            c1 = (uint32_t)((uint64_t)c0 + (fit > 1 ? fit : 1) < n ? c0 + (fit > 1 ? fit : 1) : n);
-            recs = (uint64_t)(c1 - c0) * per;
-        }
+    for (uint32_t c0 = 0, c1; c0 < n; c0 = c1) {
+        const uint64_t recs = next_pass(c0, n, h_rec_base, per, sizeof(InfRec), &c1);
         const uint32_t m = c1 - c0;
         Layout L;
         const size_t oHead = L.take((size_t)m * sizeof(InfHead)), oRec = L.take((size_t)recs * sizeof(InfRec));
@@ -1812,7 +1799,6 @@ static int launch_inflate(b2c_ctx *ctx, InfParams P, uint32_t n, uint64_t max_sr
         b2c_inflate_check_kernel<<<(m + INF_WARPS - 1) / INF_WARPS, INF_WARPS * 32, 0, st>>>(P);
         ctx->launches += 3;
         CK(cudaGetLastError());
-        c0 = c1;
     }
     return ctx_order_end(ctx, st);
 }
@@ -1842,50 +1828,20 @@ int b2c_flate_decode_chunks(b2c_ctx *ctx, int format, int flags, const void *con
     if (!ctx) return B2C_ERR_NO_DEVICE;
     if (!flate_args_ok(format, flags)) return B2C_ERR_ARG;
     if (n == 0) return B2C_OK;
-    if (n > 0xffffffffull) return B2C_ERR_ARG;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    BatchMeta meta(n);
-    const BatchMeta::Arrays &h = meta.h;
-    std::vector<uint64_t> rec_base(n + 1);
-    uint64_t inb = 0, outb = 0, nrec = 0;
-    for (size_t i = 0; i < n; i++) {
-        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
-        h.src_off[i] = inb; h.dst_off[i] = outb;
-        h.src_sizes[i] = (uint32_t)src_sizes[i];
-        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
-        rec_base[i] = nrec;
-        nrec += inf_rec_cap(src_sizes[i], h.dst_caps[i]);
-        inb += (src_sizes[i] + 15) & ~(size_t)15;
-        outb += ((size_t)h.dst_caps[i] + 15) & ~(size_t)15;
-    }
-    rec_base[n] = nrec;
-    Layout L;
-    const size_t oMeta = L.take(meta.host.size()), oBase = L.take((n + 1) * sizeof(uint64_t));
-    std::vector<uint8_t> hostMeta(L.end);
-    memcpy(hostMeta.data() + oMeta, meta.host.data(), meta.host.size());
-    memcpy(hostMeta.data() + oBase, rec_base.data(), (n + 1) * sizeof(uint64_t));
-    int rc;
-    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_meta, L.end))) return rc;
-    if ((rc = gather_h2d(ctx, srcs, src_sizes, h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, hostMeta.data(), hostMeta.size(), cudaMemcpyHostToDevice, st));
-    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p + oMeta);
-    InfParams P;
-    memset(&P, 0, sizeof(P));
-    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
-    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
-    P.out_sizes = d.res;
-    P.rec_base = ctx->d_dec_meta.at<uint64_t>(oBase);
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
+    if (rc) return rc;
+    HostBatch B(ctx, n, n, {(n + 1) * sizeof(uint64_t)});            // + the record bases
+    B.place_items(src_sizes, 0, dst_caps, 0);
+    uint64_t *rec_base = B.h_at<uint64_t>(B.ex[0]);
+    rec_base[0] = 0;
+    for (size_t i = 0; i < n; i++) rec_base[i + 1] = rec_base[i] + inf_rec_cap(src_sizes[i], B.h.dst_caps[i]);
+    if ((rc = B.stage_in(srcs, src_sizes))) return rc;
+    InfParams P = B.params<InfParams>();
+    P.rec_base = B.d_at<uint64_t>(B.ex[0]);
     P.format = format; P.multistream = !(flags & B2C_GZIP_SINGLE);
-    if ((rc = launch_inflate(ctx, P, (uint32_t)n, 0, 0, rec_base.data(), st))) return rc;
-    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::vector<size_t> lens(n, 0);
-    for (size_t i = 0; i < n; i++)
-        if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
-    return scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st);
+    if ((rc = launch_inflate(ctx, P, (uint32_t)n, 0, 0, rec_base, ctx->stream))) return rc;
+    if ((rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps);
 }
 
 // ---- stateless deflate: flate.StatelessDeflate / gzip at StatelessCompression ---------------------------------------
@@ -1963,73 +1919,44 @@ int b2c_flate_stateless_chunks(b2c_ctx *ctx, int format, int flags, const void *
     if (n == 0) return B2C_OK;
     if (n > 0xffffffffull || (dicts != nullptr) != (dict_sizes != nullptr)) return B2C_ERR_ARG;
     if (format == B2C_FLATE_GZIP && (dicts || eof)) return B2C_ERR_ARG;      // a gzip member has neither
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    BatchMeta meta(n);
-    const BatchMeta::Arrays &h = meta.h;
-    uint64_t inb = 0, outb = 0, db = 0;
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
+    if (rc) return rc;
+    // + dict offsets | dict sizes | eof flags | CRC-32 seeds | CRC-32 results; the dict tails follow, gathered on their own
+    HostBatch B(ctx, n, n, {n * 8, n * 4, n, n * 4, n * 4});
+    B.place_items(src_sizes, 0, dst_caps, 0);
+    uint64_t *dict_off = B.h_at<uint64_t>(B.ex[0]);
+    uint32_t *dict_sz = B.h_at<uint32_t>(B.ex[1]);
+    uint8_t *h_eof = B.h_at<uint8_t>(B.ex[2]);
+    uint64_t db = 0;
     uint32_t mb = 1;
-    std::vector<uint64_t> dict_off(n, 0);
-    std::vector<uint32_t> dict_sz(n, 0);
+    std::vector<const void *> dp(n);
+    std::vector<size_t> dl(n);
     for (size_t i = 0; i < n; i++) {
-        if (src_sizes[i] > 0xffffffffull) return B2C_ERR_ARG;
-        h.src_off[i] = inb; h.dst_off[i] = outb;
-        h.src_sizes[i] = (uint32_t)src_sizes[i];
-        h.dst_caps[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]);
-        const size_t dl = dicts ? (dict_sizes[i] > DFL_DICT ? DFL_DICT : dict_sizes[i]) : 0;   // only the last 8 KiB count
-        dict_off[i] = db; dict_sz[i] = (uint32_t)dl;
-        const uint32_t b = dfl_blocks(src_sizes[i], (uint32_t)dl);
+        dl[i] = dicts ? (dict_sizes[i] > DFL_DICT ? DFL_DICT : dict_sizes[i]) : 0;   // only the last 8 KiB count
+        dp[i] = dl[i] ? (const uint8_t *)dicts[i] + (dict_sizes[i] - dl[i]) : nullptr;
+        dict_off[i] = db; dict_sz[i] = (uint32_t)dl[i];
+        const uint32_t b = dfl_blocks(src_sizes[i], (uint32_t)dl[i]);
         if (b > mb) mb = b;
-        inb += (src_sizes[i] + 15) & ~(size_t)15;
-        outb += ((size_t)h.dst_caps[i] + 15) & ~(size_t)15;
-        db += (dl + 15) & ~(size_t)15;
+        db += (dl[i] + 15) & ~(size_t)15;
+        h_eof[i] = eof ? eof[i] : 1;
     }
-    Layout L;
-    const size_t oMeta = L.take(meta.host.size()), oDo = L.take(n * 8), oDs = L.take(n * 4), oEof = L.take(n),
-                 oCrc = L.take(n * 4), oCrcOut = L.take(n * 4), oDict = L.take(db + 16);
-    std::vector<uint8_t> hostMeta(oDict);
-    memcpy(hostMeta.data() + oMeta, meta.host.data(), meta.host.size());
-    memcpy(hostMeta.data() + oDo, dict_off.data(), n * 8);
-    memcpy(hostMeta.data() + oDs, dict_sz.data(), n * 4);
-    for (size_t i = 0; i < n; i++) hostMeta[oEof + i] = eof ? eof[i] : 1;
-    if (crc_in) memcpy(hostMeta.data() + oCrc, crc_in, n * 4);
-    int rc;
-    if ((rc = reserve(ctx, ctx->d_dec_in, inb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_out, outb + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_meta, L.end))) return rc;
-    if ((rc = gather_h2d(ctx, srcs, src_sizes, h.src_off, n, ctx->d_dec_in.p, (size_t)inb, st))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, hostMeta.data(), hostMeta.size(), cudaMemcpyHostToDevice, st));
+    if (crc_in) memcpy(B.h_at<uint32_t>(B.ex[3]), crc_in, n * 4);
+    const size_t oDict = B.L.take(db + 16);
+    if ((rc = B.stage_in(srcs, src_sizes))) return rc;
+    if (dicts && (rc = gather_h2d(ctx, dp.data(), dl.data(), dict_off, n, B.d_at<uint8_t>(oDict), (size_t)db, ctx->stream))) return rc;
+    DflParams P = B.params<DflParams>();
     if (dicts) {
-        std::vector<const void *> dp(n);
-        std::vector<size_t> dl(n);
-        for (size_t i = 0; i < n; i++) {
-            dl[i] = dict_sz[i];
-            dp[i] = dl[i] ? (const uint8_t *)dicts[i] + (dict_sizes[i] - dl[i]) : dicts[i];
-        }
-        if ((rc = gather_h2d(ctx, dp.data(), dl.data(), dict_off.data(), n, ctx->d_dec_meta.p + oDict, (size_t)db, st))) return rc;
+        P.dict_base = B.d_at<uint8_t>(oDict); P.dict_offsets = B.d_at<uint64_t>(B.ex[0]);
+        P.dict_sizes = B.d_at<uint32_t>(B.ex[1]);
     }
-    const BatchMeta::Arrays d = meta.at(ctx->d_dec_meta.p + oMeta);
-    DflParams P;
-    memset(&P, 0, sizeof(P));
-    P.src_base = ctx->d_dec_in.p; P.src_offsets = d.src_off; P.src_sizes = d.src_sizes;
-    if (dicts) {
-        P.dict_base = ctx->d_dec_meta.p + oDict; P.dict_offsets = ctx->d_dec_meta.at<uint64_t>(oDo);
-        P.dict_sizes = ctx->d_dec_meta.at<uint32_t>(oDs);
-    }
-    P.eof = ctx->d_dec_meta.p + oEof;
-    P.dst_base = ctx->d_dec_out.p; P.dst_offsets = d.dst_off; P.dst_caps = d.dst_caps;
-    P.out_sizes = d.res;
-    P.crc_in = crc_in ? ctx->d_dec_meta.at<uint32_t>(oCrc) : nullptr;
-    P.crc_out = ctx->d_dec_meta.at<uint32_t>(oCrcOut);
+    P.eof = B.d_at<uint8_t>(B.ex[2]);
+    P.crc_in = crc_in ? B.d_at<uint32_t>(B.ex[3]) : nullptr;
+    P.crc_out = B.d_at<uint32_t>(B.ex[4]);
     P.format = format; P.max_blocks = mb;
-    if ((rc = launch_deflate(ctx, P, (uint32_t)n, hdr, hlen, st))) return rc;
-    CK(cudaMemcpyAsync(sizes_out, d.res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    if (crc_out) CK(cudaMemcpyAsync(crc_out, P.crc_out, n * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::vector<size_t> lens(n, 0);
-    for (size_t i = 0; i < n; i++)
-        if (sizes_out[i] > 0) lens[i] = (size_t)sizes_out[i];
-    return scatter_d2h(ctx, dsts, lens.data(), h.dst_off, n, ctx->d_dec_out.p, (size_t)outb, st);
+    if ((rc = launch_deflate(ctx, P, (uint32_t)n, hdr, hlen, ctx->stream))) return rc;
+    if (crc_out) CK(cudaMemcpyAsync(crc_out, P.crc_out, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps);
 }
 
 // ---- standalone huff0 blocks ------------------------------------------------------------------------
@@ -2105,57 +2032,36 @@ static int huf_host_batch(b2c_ctx *ctx, int op, int flags, const void *const *sr
                           void *const *dsts, const size_t *dst_caps, int64_t *sizes_out, size_t n) {
     if (!ctx) return B2C_ERR_NO_DEVICE;
     if (n == 0) return B2C_OK;
-    if (n > 0xffffffffull) return B2C_ERR_ARG;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
+    int rc = HostBatch::check(ctx, n, src_sizes, 0x7fffffffull);
+    if (rc) return rc;
     size_t maxIn = 16, maxOut = 16;
     for (size_t i = 0; i < n; i++) {
-        if (src_sizes[i] > 0x7fffffffull) return B2C_ERR_ARG;
         if (src_sizes[i] > maxIn) maxIn = src_sizes[i];
         const size_t want = op == 2 ? 260 : (op == 0 ? (dst_caps[i] < src_sizes[i] ? dst_caps[i] : src_sizes[i]) : dst_caps[i]);
         if (want > maxOut) maxOut = want;
     }
     if (op == 1 && maxOut > 262144) maxOut = 262144;      // larger exact sizes are refused by the kernel (ErrTooBig class)
     const size_t inStride = (maxIn + 15) & ~(size_t)15, outStride = (maxOut + 15) & ~(size_t)15;
-    // meta: out_sizes[n] i64 | src_sizes[n] u32 | dst_sizes[n] u32
-    std::vector<uint64_t> meta(2 * n);
-    uint32_t *ss = reinterpret_cast<uint32_t *>(meta.data() + n), *ds = ss + n;
-    for (size_t i = 0; i < n; i++) { ss[i] = (uint32_t)src_sizes[i]; ds[i] = (uint32_t)(dst_caps[i] > 0xffffffffull ? 0xffffffffull : dst_caps[i]); }
-    int rc;
-    if ((rc = reserve(ctx, ctx->d_dec_in, n * inStride + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_out, n * outStride + 256))) return rc;
-    if ((rc = reserve(ctx, ctx->d_dec_meta, meta.size() * 8))) return rc;
-    for (size_t i = 0; i < n; i++)
-        if (src_sizes[i]) CK(cudaMemcpyAsync(ctx->d_dec_in.p + i * inStride, srcs[i], src_sizes[i], cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(ctx->d_dec_meta.p, meta.data(), meta.size() * 8, cudaMemcpyHostToDevice, st));
-    uint64_t *dm = ctx->d_dec_meta.at<uint64_t>(0);
-    int64_t *d_res = reinterpret_cast<int64_t *>(dm);
-    uint32_t *d_ss = reinterpret_cast<uint32_t *>(dm + n), *d_ds = d_ss + n;
+    HostBatch B(ctx, n, n);
+    B.place_items(src_sizes, inStride, dst_caps, outStride);
+    if ((rc = B.stage_in(srcs, src_sizes))) return rc;
+    uint8_t *d_in = ctx->d_dec_in.p, *d_out = ctx->d_dec_out.p;
     if (op == 0)
-        rc = b2c_huf_compress_device(ctx, flags, ctx->d_dec_in.p, inStride, d_ss, 0, ctx->d_dec_out.p, outStride, d_res, (uint32_t)n, st);
+        rc = b2c_huf_compress_device(ctx, flags, d_in, inStride, B.d.src_sizes, 0, d_out, outStride, B.d.res, (uint32_t)n, ctx->stream);
     else if (op == 1)
-        rc = b2c_huf_decompress_device(ctx, flags, ctx->d_dec_in.p, inStride, d_ss, ctx->d_dec_out.p, outStride, d_ds, d_res, (uint32_t)n, st);
+        rc = b2c_huf_decompress_device(ctx, flags, d_in, inStride, B.d.src_sizes, d_out, outStride, B.d.dst_caps, B.d.res, (uint32_t)n,
+                                       ctx->stream);
     else {
         Huf0Params P;
         memset(&P, 0, sizeof(P));
-        P.src_base = ctx->d_dec_in.p; P.src_stride = inStride; P.src_sizes = d_ss;
-        P.dst_base = ctx->d_dec_out.p; P.dst_stride = outStride; P.out_sizes = d_res; P.nchunks = (uint32_t)n;
-        b2c_huf_read_table_kernel<<<dec_grid(ctx, (uint32_t)n), DEC_WARPS * 32, DEC_SMEM_BYTES, st>>>(P);
+        P.src_base = d_in; P.src_stride = inStride; P.src_sizes = B.d.src_sizes;
+        P.dst_base = d_out; P.dst_stride = outStride; P.out_sizes = B.d.res; P.nchunks = (uint32_t)n;
+        b2c_huf_read_table_kernel<<<dec_grid(ctx, (uint32_t)n), DEC_WARPS * 32, DEC_SMEM_BYTES, ctx->stream>>>(P);
         ctx->launches += 1;
         CK(cudaGetLastError());
-        rc = B2C_OK;
     }
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(sizes_out, d_res, n * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < n; i++) {
-        if (sizes_out[i] < 0) continue;
-        const size_t bytes = op == 2 ? 260 : (size_t)sizes_out[i];
-        if (op == 0 && bytes > dst_caps[i]) { sizes_out[i] = B2C_ERR_DST_SMALL; continue; }
-        if (bytes) CK(cudaMemcpyAsync(dsts[i], ctx->d_dec_out.p + i * outStride, bytes, cudaMemcpyDeviceToHost, st));
-    }
-    CK(cudaStreamSynchronize(st));
-    return B2C_OK;
+    if (rc || (rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps, op == 2 ? 260 : 0);
 }
 int b2c_huf_compress_chunks(b2c_ctx *ctx, int flags, const void *const *srcs, const size_t *src_sizes, void *const *dsts,
                             const size_t *dst_caps, int64_t *sizes_out, size_t n) {

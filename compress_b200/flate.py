@@ -13,10 +13,9 @@ decodes at the speed of one GPU lane -- batches of many streams are what the dev
 import ctypes
 import io
 
-import numpy as np
 import torch
 
-from ._lib import lib, check, B2CError
+from ._lib import lib, check, B2CError, Context, PointerTable
 
 RAW, ZLIB, GZIP = 0, 1, 2                    # B2C_FLATE_RAW / _ZLIB / _GZIP
 GZIP_SINGLE = 1                              # B2C_GZIP_SINGLE: gzip.Reader.Multistream(false)
@@ -35,26 +34,8 @@ class ErrUnexpectedEOF(EOFError):
     """io.ErrUnexpectedEOF: the input ends inside a stream, a header or a trailer."""
 
 
-class Decoder:
+class Decoder(Context):
     """Batches of raw DEFLATE / zlib / gzip streams decoded on one GPU."""
-
-    def __init__(self, device=0):
-        if lib.b2c_device_count() <= 0:
-            raise B2CError("no CUDA device")
-        self._ctx = lib.b2c_ctx_create(device, 0)
-        if not self._ctx:
-            raise B2CError("b2c_ctx_create failed")
-
-    def close(self):
-        if self._ctx:
-            lib.b2c_ctx_destroy(self._ctx)
-            self._ctx = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
 
     def decode_device(self, src, src_sizes, src_stride, dst=None, dst_cap=1 << 16, out_sizes=None, format=GZIP,
                       multistream=True, src_offsets=None):
@@ -78,20 +59,12 @@ class Decoder:
     def decode_chunks(self, inputs, caps, format=GZIP, multistream=True):
         """Host buffers: inputs[i] decoded into at most caps[i] bytes.  Returns (outputs, codes): outputs[i] is the content
         (None on error), codes[i] its length or a negative B2C_ERR_* code."""
-        n = len(inputs)
-        if n == 0:
+        if not inputs:
             return [], []
-        bufs = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(1, dtype=np.uint8) for b in inputs]
-        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(b) for b in inputs])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
-        res = (ctypes.c_int64 * n)()
-        check(lib.b2c_flate_decode_chunks(self._ctx, format, 0 if multistream else GZIP_SINGLE, srcs, ssz, dsts, dcap, res, n),
-              self._ctx)
-        codes = [int(r) for r in res]
-        return [outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes
+        t = PointerTable(inputs, caps)
+        check(lib.b2c_flate_decode_chunks(self._ctx, format, 0 if multistream else GZIP_SINGLE, t.srcs, t.ssz, t.dsts, t.dcap,
+                                          t.res, t.n), self._ctx)
+        return t.results()
 
     def decode_all(self, data, format, multistream=True):
         """One input of unknown content size: the destination starts at 4x the input (at least 64 KiB) and doubles while it
@@ -150,26 +123,8 @@ def StatelessBound(n, dict_len=0):
     return int(lib.b2c_flate_stateless_bound(n, dict_len))
 
 
-class Encoder:
+class Encoder(Context):
     """Batches of flate.StatelessDeflate calls (raw) or gzip members at StatelessCompression, encoded on one GPU."""
-
-    def __init__(self, device=0):
-        if lib.b2c_device_count() <= 0:
-            raise B2CError("no CUDA device")
-        self._ctx = lib.b2c_ctx_create(device, 0)
-        if not self._ctx:
-            raise B2CError("b2c_ctx_create failed")
-
-    def close(self):
-        if self._ctx:
-            lib.b2c_ctx_destroy(self._ctx)
-            self._ctx = None
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
 
     def encode_device(self, src, src_sizes, src_stride, dst=None, dst_cap=None, out_sizes=None, format=RAW, eof=None,
                       dict=None, dict_offsets=None, dict_sizes=None, header=b"", crc_in=None, crc_out=None,
@@ -206,31 +161,18 @@ class Encoder:
             return [], [], []
         if caps is None:
             caps = [StatelessBound(len(b), MAX_STATELESS_DICT) + len(header) + 10 for b in inputs]
-        keep = []
-
-        def arr(bs):
-            a = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(1, dtype=np.uint8) for b in bs]
-            keep.append(a)
-            return (ctypes.c_void_p * n)(*[x.ctypes.data for x in a])
-        srcs = arr(inputs)
-        ssz = (ctypes.c_size_t * n)(*[len(b) for b in inputs])
-        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
+        t = PointerTable(inputs, caps)
         eofs = None if eof is None else (ctypes.c_uint8 * n)(*[1 if e else 0 for e in eof])
         dp = dsz = None
         if dicts is not None:
             dl = [d or b"" for d in dicts]
-            dp = arr(dl)
+            dp = t.pointers(dl)
             dsz = (ctypes.c_size_t * n)(*[len(d) for d in dl])
         cin = None if crc_in is None else (ctypes.c_uint32 * n)(*crc_in)
         cout = (ctypes.c_uint32 * n)()
-        res = (ctypes.c_int64 * n)()
-        check(lib.b2c_flate_stateless_chunks(self._ctx, format, 0, srcs, ssz, eofs, dp, dsz, bytes(header), len(header),
-                                             dsts, dcap, res, cin, cout, n), self._ctx)
-        codes = [int(r) for r in res]
-        return ([outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes,
-                [int(c) for c in cout])
+        check(lib.b2c_flate_stateless_chunks(self._ctx, format, 0, t.srcs, t.ssz, eofs, dp, dsz, bytes(header), len(header),
+                                             t.dsts, t.dcap, t.res, cin, cout, n), self._ctx)
+        return (*t.results(), [int(c) for c in cout])
 
 
 _enc = None

@@ -9,7 +9,7 @@ import ctypes
 import numpy as np
 import torch
 
-from ._lib import lib, check, B2CError
+from ._lib import lib, check, B2CError, Context, PointerTable
 
 BlockSizeMax = (1 << 18) - 1
 
@@ -33,25 +33,10 @@ class ErrCorrupt(B2CError):
 _ERR = {-1: ErrIncompressible, -2: ErrUseRLE, -3: ErrTooBig, -5: ErrCorrupt}
 
 
-class Codec:
+class Codec(Context):
     def __init__(self, device=0):
-        if not torch.cuda.is_available() or lib.b2c_device_count() == 0:
-            raise B2CError("no CUDA device: compress_b200 has no CPU fallback")
+        super().__init__(device)
         self.dev = torch.device("cuda", device)
-        self._ctx = lib.b2c_ctx_create(device, 0)
-        if not self._ctx:
-            raise B2CError("b2c_ctx_create failed")
-
-    def close(self):
-        if self._ctx:
-            lib.b2c_ctx_destroy(self._ctx)
-            self._ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- device-resident batches ----------------------------------------------------------------
     def compress_device(self, src, stride, sizes=None, four=True, dst=None, out_sizes=None):
@@ -118,40 +103,29 @@ class Codec:
         return [(dsth[i, :outs[i]].tobytes() if outs[i] >= 0 else None, int(outs[i])) for i in range(n)]
 
     # ---- host-buffer C-ABI calls (what a cgo shim binds) ------------------------------------------------------
-    def _host(self, fn, blobs, caps, *pre):
-        n = len(blobs)
-        bufs = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(0, dtype=np.uint8) for b in blobs]
-        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(b) for b in blobs])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        res = (ctypes.c_int64 * n)()
-        if caps is not None and fn is not lib.b2c_huf_read_table:
-            dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
-            check(fn(self._ctx, *pre, srcs, ssz, dsts, dcap, res, n), self._ctx)
-        else:
-            check(fn(self._ctx, srcs, ssz, dsts, res, n), self._ctx)
-        return outs, [int(r) for r in res]
+    def _host(self, fn, blobs, caps, four):
+        """-> list of (bytes or None, code)."""
+        if not blobs:
+            return []
+        t = PointerTable(blobs, caps)
+        check(fn(self._ctx, 1 if four else 0, t.srcs, t.ssz, t.dsts, t.dcap, t.res, t.n), self._ctx)
+        return list(zip(*t.results()))
 
     def compress_chunks(self, blocks, four=True):
         """b2c_huf_compress_chunks: -> list of (bytes or None, code)."""
-        if not blocks:
-            return []
-        outs, codes = self._host(lib.b2c_huf_compress_chunks, blocks, [len(b) + 16 for b in blocks], 1 if four else 0)
-        return [(outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None, codes[i]) for i in range(len(blocks))]
+        return self._host(lib.b2c_huf_compress_chunks, blocks, [len(b) + 16 for b in blocks], four)
 
     def decompress_chunks(self, blocks, dst_sizes, four=True):
-        if not blocks:
-            return []
-        outs, codes = self._host(lib.b2c_huf_decompress_chunks, blocks, dst_sizes, 1 if four else 0)
-        return [(outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None, codes[i]) for i in range(len(blocks))]
+        return self._host(lib.b2c_huf_decompress_chunks, blocks, dst_sizes, four)
 
     def ReadTable(self, data):
         """huff0.ReadTable(in, nil) (huff0/decompress.go:29): -> (code length per symbol [256], tableLog, remaining input)."""
-        outs, codes = self._host(lib.b2c_huf_read_table, [data], [260])
-        if codes[0] < 0:
-            raise _ERR.get(codes[0], B2CError)(lib.b2c_strerror(codes[0]).decode())
-        row = outs[0]
+        t = PointerTable([data], [260])
+        check(lib.b2c_huf_read_table(self._ctx, t.srcs, t.ssz, t.dsts, t.res, t.n), self._ctx)
+        code = int(t.res[0])
+        if code < 0:
+            raise _ERR.get(code, B2CError)(lib.b2c_strerror(code).decode())
+        row = t.outs[0]
         used = int(row[2]) | (int(row[3]) << 8)
         return [int(x) for x in row[4:260]], int(row[0]), bytes(data)[used:]
 

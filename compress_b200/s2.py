@@ -14,7 +14,7 @@ import ctypes
 import numpy as np
 import torch
 
-from ._lib import lib, check, B2CError
+from ._lib import lib, check, B2CError, Context, PointerTable
 from . import s2_index
 from .s2_index import Index, IndexStream, RemoveIndexHeaders, RestoreIndexHeaders   # noqa: F401  (s2/index.go)
 
@@ -98,26 +98,10 @@ def ConcatBlocks(blocks, dst=None):
     return bytes(out) if dst is None else out
 
 
-class Codec:
+# class Codec: batches of S2 blocks on one GPU.  The helpers above need neither torch nor the library, and
+# tests/test_s2_stream_model.py runs them on their own by cutting this file at this line's first words.
+class Codec(Context):
     """Batch S2 block encoder/decoder on one GPU."""
-
-    def __init__(self, device=0):
-        if not torch.cuda.is_available() or lib.b2c_device_count() == 0:
-            raise B2CError("no CUDA device: compress_b200 has no CPU fallback")
-        self._ctx = lib.b2c_ctx_create(device, 0)
-        if not self._ctx:
-            raise B2CError("b2c_ctx_create failed")
-
-    def close(self):
-        if self._ctx:
-            lib.b2c_ctx_destroy(self._ctx)
-            self._ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     @property
     def launches(self):
@@ -165,17 +149,9 @@ class Codec:
         return f
 
     def _host(self, fn, blobs, caps, *pre):
-        n = len(blobs)
-        bufs = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(0, dtype=np.uint8) for b in blobs]
-        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(b) for b in blobs])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
-        res = (ctypes.c_int64 * n)()
-        check(fn(self._ctx, *pre, srcs, ssz, dsts, dcap, res, n), self._ctx)
-        codes = [int(r) for r in res]
-        return [outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes
+        t = PointerTable(blobs, caps)
+        check(fn(self._ctx, *pre, t.srcs, t.ssz, t.dsts, t.dcap, t.res, t.n), self._ctx)
+        return t.results()
 
     def encode_blocks(self, blocks, snappy=False, better=False, best=False):
         level = _level(better, best)
@@ -243,20 +219,13 @@ class Codec:
     def convert_lz4_blocks(self, blocks, caps, lz4s=False, snappy=False):
         """Convert LZ4 (or LZ4s) blocks; caps[i] = slot capacity.  Returns (outs, codes, ns): outs[i] = uvarint(n) + the S2
         (Snappy) body or None, codes[i] = its size or a negative error, ns[i] = the decoded size."""
-        n = len(blocks)
-        if n == 0:
+        if not blocks:
             return [], [], []
-        bufs = [np.frombuffer(bytes(b), dtype=np.uint8) if len(b) else np.zeros(1, dtype=np.uint8) for b in blocks]
-        outs = [np.empty(max(int(c), 1), dtype=np.uint8) for c in caps]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(b) for b in blocks])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[int(c) for c in caps])
-        res, dec = (ctypes.c_int64 * n)(), (ctypes.c_int64 * n)()
-        check(lib.b2c_s2_convert_lz4_chunks(self._ctx, 1 if lz4s else 0, FLAG_SNAPPY if snappy else 0, srcs, ssz, dsts, dcap,
-                                            res, dec, n), self._ctx)
-        codes = [int(r) for r in res]
-        return [outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes, [int(x) for x in dec]
+        t = PointerTable(blocks, caps)
+        dec = (ctypes.c_int64 * t.n)()
+        check(lib.b2c_s2_convert_lz4_chunks(self._ctx, 1 if lz4s else 0, FLAG_SNAPPY if snappy else 0, t.srcs, t.ssz, t.dsts,
+                                            t.dcap, t.res, dec, t.n), self._ctx)
+        return (*t.results(), [int(x) for x in dec])
 
     def convert_lz4_device(self, src, src_sizes, src_stride, lz4s=False, snappy=False, dst=None, dst_cap=None, out_sizes=None,
                            decoded=None, src_offsets=None, dst_offsets=None, dst_stride=None):

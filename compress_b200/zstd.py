@@ -25,15 +25,22 @@ FLAG_CRC = 1
 FLAG_FRAME = 2
 
 
-class Encoder:
+def _raise_first(results, what):
+    """The outputs of a batch, or B2CError for its first failing item."""
+    outs, codes = results
+    for i, c in enumerate(codes):
+        if c < 0:
+            raise B2CError(f"{what} {i}: {lib.b2c_strerror(c).decode()}")
+    return outs
+
+
+class Encoder(_lib.Context):
     """zstd.Encoder on one GPU: batches of independent blocks (one-block frames: encode_device / encode_chunks /
     encode_packed) and frame mode (encode_frames / EncodeAll: one multi-block frame per input, blocks with history).
     padding: WithEncoderPadding -- EncodeAll output and a Writer's total are brought to a multiple of it with a skippable
     frame (zstd/encoder_options.go, zstd/frameenc.go:96-137)."""
 
     def __init__(self, level=SpeedFastest, crc=True, device=0, max_chunks=4096, padding=0):
-        if not torch.cuda.is_available() or lib.b2c_device_count() == 0:
-            raise B2CError("no CUDA device: compress_b200 has no CPU fallback")
         if level not in BLOCK:
             raise B2CError("levels on the GPU path: SpeedFastest, SpeedDefault, SpeedBetterCompression")
         self.level = level
@@ -45,20 +52,7 @@ class Encoder:
         if padding < 0 or padding > 1 << 30:
             raise B2CError("padding must be in [0, 1 GiB]")
         self.padding = padding
-        self._ctx = lib.b2c_ctx_create(device, max_chunks)
-        if not self._ctx:
-            raise B2CError("b2c_ctx_create failed")
-
-    def close(self):
-        if self._ctx:
-            lib.b2c_ctx_destroy(self._ctx)
-            self._ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(device, max_chunks)
 
     @property
     def launches(self):
@@ -128,24 +122,11 @@ class Encoder:
     # ---- host buffers (what the cgo shim calls) -----------------------------------------------
     def encode_chunks(self, chunks):
         """chunks: list of bytes-like (each at most the level's block size).  Returns list of encoded frames (bytes)."""
-        n = len(chunks)
-        if n == 0:
+        if not chunks:
             return []
-        bufs = [np.frombuffer(c, dtype=np.uint8) if len(c) else np.zeros(0, dtype=np.uint8) for c in chunks]
-        outs = [np.empty(self.MaxEncodedSize(len(c)) + 16, dtype=np.uint8) for c in chunks]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(c) for c in chunks])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[o.size for o in outs])
-        res = (ctypes.c_int64 * n)()
-        rc = lib.b2c_zstd_encode_chunks(self._ctx, self.level, self.flags, srcs, ssz, dsts, dcap, res, n)
-        check(rc, self._ctx)
-        out = []
-        for i in range(n):
-            if res[i] < 0:
-                raise B2CError(f"chunk {i}: {lib.b2c_strerror(int(res[i])).decode()}")
-            out.append(outs[i][: res[i]].tobytes())
-        return out
+        t = _lib.PointerTable(chunks, [self.MaxEncodedSize(len(c)) + 16 for c in chunks])
+        check(lib.b2c_zstd_encode_chunks(self._ctx, self.level, self.flags, t.srcs, t.ssz, t.dsts, t.dcap, t.res, t.n), self._ctx)
+        return _raise_first(t.results(), "chunk")
 
     def encode_packed(self, src, dst=None, chunk=None):
         """src: contiguous host buffer (bytes / numpy / CPU torch tensor, ideally pinned).  Returns
@@ -197,24 +178,12 @@ class Encoder:
     def encode_frames(self, inputs):
         """inputs: list of bytes-like of any size.  Returns one zstd frame (bytes) per input: Encoder.EncodeAll applied to
         each, all blocks of all inputs in one device batch."""
-        n = len(inputs)
-        if n == 0:
+        if not inputs:
             return []
-        bufs = [np.frombuffer(c, dtype=np.uint8) if len(c) else np.zeros(0, dtype=np.uint8) for c in inputs]
-        outs = [np.empty(self.FrameBound(len(c)) + 16, dtype=np.uint8) for c in inputs]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(c) for c in inputs])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[o.size for o in outs])
-        res = (ctypes.c_int64 * n)()
-        rc = lib.b2c_zstd_encode_frames(self._ctx, self.level, self.flags & FLAG_CRC, srcs, ssz, dsts, dcap, res, n)
-        check(rc, self._ctx)
-        out = []
-        for i in range(n):
-            if res[i] < 0:
-                raise B2CError(f"input {i}: {lib.b2c_strerror(int(res[i])).decode()}")
-            out.append(outs[i][: res[i]].tobytes())
-        return out
+        t = _lib.PointerTable(inputs, [self.FrameBound(len(c)) + 16 for c in inputs])
+        check(lib.b2c_zstd_encode_frames(self._ctx, self.level, self.flags & FLAG_CRC, t.srcs, t.ssz, t.dsts, t.dcap, t.res, t.n),
+              self._ctx)
+        return _raise_first(t.results(), "input")
 
     def EncodeAll(self, src, dst=None, single_frame=True):
         """EncodeAll will encode all input in src and append it to dst (zstd/encoder.go:715-729).  As in the reference the
@@ -318,28 +287,13 @@ ErrCorrupt = -5
 ErrDecoderSizeExceeded = -4
 
 
-class Decoder:
+class Decoder(_lib.Context):
     """zstd.Decoder for batches of independent streams on one GPU (staged kernels; a one-warp decoder for the rest)."""
 
     def __init__(self, device=0, max_decoded=64 << 20):
-        if not torch.cuda.is_available() or lib.b2c_device_count() == 0:
-            raise B2CError("no CUDA device: compress_b200 has no CPU fallback")
         self.device = device
         self.max_decoded = max_decoded       # WithDecoderMaxMemory analogue for DecodeAll without a known size
-        self._ctx = lib.b2c_ctx_create(device, 0)
-        if not self._ctx:
-            raise B2CError("b2c_ctx_create failed")
-
-    def close(self):
-        if self._ctx:
-            lib.b2c_ctx_destroy(self._ctx)
-            self._ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(device)
 
     @property
     def launches(self):
@@ -392,22 +346,11 @@ class Decoder:
 
     def decode_chunks(self, streams, caps=None):
         """streams: list of bytes-like zstd streams.  Returns (list of bytes or None, list of codes)."""
-        n = len(streams)
-        if n == 0:
+        if not streams:
             return [], []
-        if caps is None:
-            caps = [self.max_decoded] * n
-        bufs = [np.frombuffer(bytes(c), dtype=np.uint8) if len(c) else np.zeros(0, dtype=np.uint8) for c in streams]
-        outs = [np.empty(max(int(cp), 1), dtype=np.uint8) for cp in caps]
-        srcs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        ssz = (ctypes.c_size_t * n)(*[len(c) for c in streams])
-        dsts = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
-        dcap = (ctypes.c_size_t * n)(*[int(cp) for cp in caps])
-        res = (ctypes.c_int64 * n)()
-        rc = lib.b2c_zstd_decode_chunks(self._ctx, srcs, ssz, dsts, dcap, res, n)
-        check(rc, self._ctx)
-        codes = [int(r) for r in res]
-        return [outs[i][:codes[i]].tobytes() if codes[i] >= 0 else None for i in range(n)], codes
+        t = _lib.PointerTable(streams, [self.max_decoded] * len(streams) if caps is None else caps)
+        check(lib.b2c_zstd_decode_chunks(self._ctx, t.srcs, t.ssz, t.dsts, t.dcap, t.res, t.n), self._ctx)
+        return t.results()
 
     def DecodeAll(self, input, dst=None, size_hint=None):
         """DecodeAll decodes a full zstd stream and appends it to dst (zstd/decoder.go:311-385)."""
