@@ -1959,6 +1959,100 @@ int b2c_flate_stateless_chunks(b2c_ctx *ctx, int format, int flags, const void *
     return B.scatter(dsts, sizes_out, dst_caps);
 }
 
+// ---- BestSpeed: flate.NewWriter(w, 1), zlib / gzip.NewWriterLevel(w, BestSpeed) ------------------------------------
+// One lane per input.  Its scratch -- a 2^15-entry int32 table, a window's tokens, a DflSlot and a DflState, about 385 KiB
+// -- is in d_dfl; a batch whose lanes need more than kDflL1PassBytes runs in passes over its inputs, each pass's tables
+// zeroed before it.
+static const uint64_t kDflL1PassBytes = (uint64_t)4 << 30;
+static const size_t kDflL1LaneBytes = DFL_L1_TABLE * 4 + DFL_L1_TOKENS * 4 + sizeof(DflSlot) + sizeof(DflState);
+// The bound.  storeFast writes each window as one block, and no block is more than 176 bytes longer than the window:
+//  - stored: 4 bytes of LEN / NLEN, the 3-bit header and its byte padding, and up to 15 bits of the EOB the block before
+//    owed: len + 8.
+//  - dynamic: chosen only when its exact size (reuseSize or the new table's header and codes, or the fixed size) is below
+//    the stored size, (len + 5) * 8 bits; with the owed EOB, len + 8.
+//  - Huffman-only: chosen on an estimate, estBits < (len + 5) * 8, where estBits counts the window's codes and the EOB at
+//    their real lengths plus either the table in force's real header (reuse) or a guessed 560-bit header.  A new header
+//    for 257 literal and 1 offset code lengths has 17 + 19 * 3 bits and at most 7 bits per code length (repeat codes
+//    carry fewer per length), 1 880 bits, so the block is at most 1 320 bits over its estimate: with the owed EOB,
+//    len + 5 + 168 < len + 176.
+// Close adds the final empty block, its owed EOB and the last partial byte: 4 bytes.  zlib adds 6 bytes, gzip hlen + 8.
+size_t b2c_flate_best_speed_bound(size_t n) { return n + 176 * (n / DFL_L1_WINDOW + 1) + 4; }
+
+static int launch_best_speed(b2c_ctx *ctx, DflParams P, uint32_t n, const void *hdr, size_t hlen, cudaStream_t st) {
+    const uint32_t maxLanes = (uint32_t)(kDflL1PassBytes / kDflL1LaneBytes), passes = (n + maxLanes - 1) / maxLanes,
+                   lanes = (n + passes - 1) / passes;
+    Layout L;
+    const size_t oTab = L.take((size_t)lanes * DFL_L1_TABLE * 4), oTok = L.take((size_t)lanes * DFL_L1_TOKENS * 4),
+                 oSlots = L.take((size_t)lanes * sizeof(DflSlot)), oState = L.take((size_t)lanes * sizeof(DflState)),
+                 oHdr = L.take(hlen ? hlen : 1);
+    { int r = reserve(ctx, ctx->d_dfl, L.end); if (r) return r; }
+    { int r = ctx_order_begin(ctx, st); if (r) return r; }
+    int32_t *tables = ctx->d_dfl.at<int32_t>(oTab);
+    P.tokens = ctx->d_dfl.at<uint32_t>(oTok);
+    P.slots = ctx->d_dfl.at<DflSlot>(oSlots);
+    P.state = ctx->d_dfl.at<DflState>(oState);
+    P.hdr = ctx->d_dfl.p + oHdr; P.hlen = (uint32_t)hlen;
+    if (hlen) CK(cudaMemcpyAsync(ctx->d_dfl.p + oHdr, hdr, hlen, cudaMemcpyHostToDevice, st));
+    for (uint32_t i0 = 0; i0 < n; i0 += lanes) {
+        const uint32_t i1 = n - i0 < lanes ? n : i0 + lanes;
+        CK(cudaMemsetAsync(tables, 0, (size_t)(i1 - i0) * DFL_L1_TABLE * 4, st));
+        b2c_deflate_l1_kernel<<<(i1 - i0 + DFL_ENCODE_LANES - 1) / DFL_ENCODE_LANES, DFL_ENCODE_LANES, 0, st>>>(P, tables, i0, i1);
+        ctx->launches += 1;
+        CK(cudaGetLastError());
+    }
+    b2c_deflate_l1_check_kernel<<<(n + DFL_CRC_WARPS - 1) / DFL_CRC_WARPS, DFL_CRC_WARPS * 32, 0, st>>>(P, n);
+    ctx->launches += 1;
+    CK(cudaGetLastError());
+    return ctx_order_end(ctx, st);
+}
+static bool best_speed_args_ok(int format, int flags, const void *hdr, size_t hlen) {
+    if (flags != 0 || (format != B2C_FLATE_RAW && format != B2C_FLATE_ZLIB && format != B2C_FLATE_GZIP)) return false;
+    if (format == B2C_FLATE_GZIP) return hdr && hlen >= 10 && hlen < (1u << 20);
+    return hlen == 0;
+}
+
+int b2c_flate_best_speed_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                                const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, const void *hdr, size_t hlen,
+                                void *d_dst, size_t dst_stride, const uint64_t *d_dst_offsets, uint32_t dst_cap,
+                                int64_t *d_out_sizes, uint32_t *d_check_out, uint32_t nchunks, void *stream) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if (!best_speed_args_ok(format, flags, hdr, hlen)) return B2C_ERR_ARG;
+    if (!d_src_sizes || !d_out_sizes || src_stride == 0 || src_stride > 0xffffffffull) return B2C_ERR_ARG;
+    if (nchunks == 0) return B2C_OK;
+    CK(cudaSetDevice(ctx->device));
+    DflParams P;
+    memset(&P, 0, sizeof(P));
+    P.src_base = (const uint8_t *)d_src; P.src_stride = src_stride; P.src_offsets = d_src_offsets; P.src_sizes = d_src_sizes;
+    P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_offsets = d_dst_offsets; P.dst_cap = dst_cap;
+    P.out_sizes = d_out_sizes; P.crc_out = d_check_out;
+    P.format = format;
+    return launch_best_speed(ctx, P, nchunks, hdr, hlen, (cudaStream_t)stream);
+}
+
+int b2c_flate_best_speed_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                                const void *hdr, size_t hlen, void *const *dsts, const size_t *dst_caps, int64_t *sizes_out,
+                                uint32_t *check_out, size_t n) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if (!best_speed_args_ok(format, flags, hdr, hlen)) return B2C_ERR_ARG;
+    if (n == 0) return B2C_OK;
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
+    if (rc) return rc;
+    // an input over the cap is not staged: the lane refuses it from its size alone
+    std::vector<size_t> staged(src_sizes, src_sizes + n);
+    for (size_t i = 0; i < n; i++) if (staged[i] > DFL_L1_MAX_INPUT) staged[i] = 0;
+    HostBatch B(ctx, n, n, {n * 4});                                  // + the checksums
+    B.place_items(staged.data(), 0, dst_caps, 0);
+    for (size_t i = 0; i < n; i++) B.h.src_sizes[i] = (uint32_t)src_sizes[i];
+    if ((rc = B.stage_in(srcs, staged.data()))) return rc;
+    DflParams P = B.params<DflParams>();
+    P.crc_out = B.d_at<uint32_t>(B.ex[0]);
+    P.format = format;
+    if ((rc = launch_best_speed(ctx, P, (uint32_t)n, hdr, hlen, ctx->stream))) return rc;
+    if (check_out) CK(cudaMemcpyAsync(check_out, P.crc_out, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps);
+}
+
 // ---- standalone huff0 blocks ------------------------------------------------------------------------
 int b2c_huf_compress_device(b2c_ctx *ctx, int flags, const void *d_src, size_t src_stride, const uint32_t *d_sizes,
                             uint32_t size_all, void *d_dst, size_t dst_stride, int64_t *d_out_sizes, uint32_t nchunks,

@@ -22,7 +22,7 @@ namespace b2c {
 constexpr uint32_t DFL_BLOCK0 = 32767, DFL_STEP = 24575, DFL_DICT = 8192;
 constexpr uint32_t DFL_SLOT_TOKENS = 32768;            // tokens of one block, EOB included (a block is at most 32767 bytes)
 constexpr int DFL_LIT = 286, DFL_OFF = 30, DFL_EOB = 256, DFL_CG = 19;
-constexpr int DFL_FMT_RAW = 0, DFL_FMT_GZIP = 2;
+constexpr int DFL_FMT_RAW = 0, DFL_FMT_GZIP = 2;      // and DFL_FMT_ZLIB (BestSpeed only)
 
 struct DflSlot {                                       // one parsed block
     uint32_t n, pad[3];
@@ -486,7 +486,9 @@ B2C_DEV int dfl_estimated_bits(const DflSlot *s, uint32_t ntok, const uint16_t *
     return (int)shannon + bits;
 }
 
-// writeBlockDynamic (huffman_bit_writer.go:620-765) for a parsed block; logNewTablePenalty is 0 in the stateless path
+// writeBlockDynamic (huffman_bit_writer.go:620-765) for a parsed block.  PEN is the writer's logNewTablePenalty: 0 in the
+// stateless path (a pooled writer), 7 at BestSpeed (deflate.go:803-808).
+template <int PEN>
 B2C_DEV void dfl_block_dynamic(DflWriter &w, const DflSlot *s, const uint32_t *toks, bool eof, const uint8_t *input,
                                uint32_t inlen, bool sync) {
     DflState *st = w.st;
@@ -536,7 +538,7 @@ B2C_DEV void dfl_block_dynamic(DflWriter &w, const DflSlot *s, const uint32_t *t
     int size = 0;
     if (w.lastHeader > 0) {
         int newSize = w.lastHeader + dfl_estimated_bits(s, ntok, lf + 256);
-        newSize += (int)(w.lit()->codes[DFL_EOB] & 0xff) + newSize;
+        newSize += (int)(w.lit()->codes[DFL_EOB] & 0xff) + (newSize >> PEN);
         const int reuseSize = dfl_bitlen(w.lit()->codes, lf, 289) + dfl_bitlen(st->off.codes, of, 32) + extraBits;
         if (newSize < reuseSize) { w.code(w.lit()->codes[DFL_EOB]); size = newSize; w.lastHeader = 0; }
         else size = reuseSize;
@@ -573,7 +575,8 @@ B2C_DEV void dfl_block_dynamic(DflWriter &w, const DflSlot *s, const uint32_t *t
     w.tokens(toks, s->n, [lc](uint32_t c) { return lc[c]; }, [oc](uint32_t c) { return oc[c]; }, sync);
 }
 
-// writeBlockHuff (huffman_bit_writer.go:987-1174); huffOffset is one code of length 1 for offset 0
+// writeBlockHuff (huffman_bit_writer.go:987-1174); huffOffset is one code of length 1 for offset 0; PEN as above
+template <int PEN>
 B2C_DEV void dfl_block_huff(DflWriter &w, bool eof, const uint8_t *input, uint32_t inlen, bool sync) {
     DflState *st = w.st;
     uint16_t *lf = st->literalFreq;
@@ -598,7 +601,7 @@ B2C_DEV void dfl_block_huff(DflWriter &w, bool eof, const uint8_t *input, uint32
     if (estBits < 0x7fffffff) {
         estBits += w.lastHeader;
         if (w.lastHeader == 0) estBits += 70 * 8;
-        estBits += estBits;
+        estBits += estBits >> PEN;
     }
     if (storable && ssize <= estBits) { w.stored(input, inlen, eof); return; }
     if (w.lastHeader > 0 && estBits < dfl_reuse_bits(w.lit()->codes, lf, 256)) {
@@ -654,8 +657,8 @@ B2C_DEV void dfl_encode_lane(const DflParams &P, uint32_t i) {
         const bool last = k + 1 == nb, isEof = eof && last;
         const uint8_t *blk = in + b.start;
         if (s->n == 0) w.stored(blk, b.len, isEof);
-        else if ((int)s->n > (int)b.len - (int)(b.len >> 4)) dfl_block_huff(w, isEof, blk, b.len, last);
-        else dfl_block_dynamic(w, s, toks, isEof, blk, b.len, last);
+        else if ((int)s->n > (int)b.len - (int)(b.len >> 4)) dfl_block_huff<0>(w, isEof, blk, b.len, last);
+        else dfl_block_dynamic<0>(w, s, toks, isEof, blk, b.len, last);
     }
     if (ends) {
         if (eof && n == 0) { w.stored_header(0, true); w.flush(); }
@@ -689,6 +692,177 @@ B2C_DEV void dfl_crc_warp(const DflParams &P, uint32_t i, const uint32_t *tab, u
     P.out_sizes[i] = r + 8;
 }
 
+// ---- BestSpeed: flate.NewWriter(w, BestSpeed) for Writes then Close (deflate.go:713-880, level1.go, fast_encoder.go),
+// raw or inside the zlib / gzip writers' framing, one lane per input.
+// The compressor fills a 65 535-byte window and runs storeFast each time it is full and more bytes arrive; Close runs it
+// once more with sync set (deflate.go:755-770, :865-880).  Without Flush the blocks therefore depend on the byte count
+// alone: consecutive 65 535-byte windows, the last one possibly shorter and the only one written with sync.  fastEncL1
+// parses each window with the table and history the windows before it left, so parse and bit writer share the lane.
+constexpr int32_t DFL_L1_WINDOW = 65535;               // maxStoreBlockSize; also e.cur's start
+constexpr int32_t DFL_L1_HIST = 5 * DFL_L1_WINDOW;     // allocHistory: cap(e.hist)
+constexpr int32_t DFL_L1_MAXOFF = 32768;               // maxMatchOffset
+constexpr uint32_t DFL_L1_TABLE = 1u << 15;            // tableSize, int32 entries
+constexpr uint32_t DFL_L1_TOKENS = 65536;              // tokens of one window: at most one per byte
+constexpr int DFL_FMT_ZLIB = 1;
+// The input cap.  The table holds e.cur + hist position; e.cur starts at 65 535 and grows only when addBlock moves the
+// history down, by at most the bytes added, so it stays <= 65 535 + n.  With n <= 2^30 that is below bufferReset
+// (2^31 - 6 * 65 535 - 1, fast_encoder.go:49), Encode's table shift (level1.go:29-49) never runs, and every position
+// below fits an int32.
+constexpr uint32_t DFL_L1_MAX_INPUT = 1u << 30;
+// The 16-bit counts of DflSlot and DflState cannot overflow: a window has at most 65 535 bytes and every token covers at
+// least one of them, so litHist / extraHist / offHist, and literalFreq / offsetFreq built from them, count at most 65 535
+// (the EOB and the empty-offset 1 have slots of their own); writeBlockHuff's literalFreq counts the window's bytes, at most
+// 65 535 per value; codegenFreq counts at most 320 code lengths.  The reference keeps the same uint16 counts.
+
+// Little-endian 8 bytes at p from the aligned words that hold them.  The second word is read only when p is unaligned,
+// and then it holds p[7]: no load touches a word outside the bytes asked for.
+B2C_DEV uint64_t dfl_ld64u(const uint8_t *p) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    const uint64_t *w = reinterpret_cast<const uint64_t *>(a & ~(uintptr_t)7);
+    const uint32_t sh = (uint32_t)(a & 7) * 8;
+    const uint64_t lo = w[0];
+    return sh ? (lo >> sh) | (w[1] << (64 - sh)) : lo;
+}
+B2C_DEV uint32_t dfl_l1_hash(uint64_t u) { return (uint32_t)(((u << 24) * 889523592379ull) >> 49); }  // hashLen(u, 15, 5)
+// matchLen(in[a:end], in[b:]) (matchlen_generic.go), b < a
+B2C_DEV int32_t dfl_l1_matchlen(const uint8_t *in, int32_t a, int32_t b, int32_t end) {
+    int32_t k = 0;
+    for (; a + k + 8 <= end; k += 8) {
+        const uint64_t x = dfl_ld64u(in + a + k) ^ dfl_ld64u(in + b + k);
+        if (x) return k + (__ffsll((long long)x) - 1) / 8;
+    }
+    while (a + k < end && in[a + k] == in[b + k]) k++;
+    return k;
+}
+
+// fastEncL1.Encode (level1.go:51-215) of the window in[bs, be) whose e.hist starts at in[hs] (addBlock,
+// fast_encoder.go:81-101).  The input is read in place: positions are the input's, and a table entry e.cur + hist position
+// is 65 535 + input position, since e.cur - hs starts at 65 535 and a move adds the same shift to both.  e.hist's bounds
+// are kept exactly: backward extension stops at hs (`t > 0`), and matches end at be (e.hist ends with the window).
+B2C_DEV void dfl_l1_parse(const uint8_t *in, int32_t hs, int32_t bs, int32_t be, DflTok &dst, int32_t *table) {
+    const int32_t sLimit = be - 11;                    // len(src) - inputMargin
+    int32_t s = bs, nextEmit = bs, nextS, t;
+    uint64_t cv = dfl_ld64u(in + s);
+    for (;;) {
+        for (;;) {                                     // two probes per step, skipping faster the longer nothing matches
+            uint32_t nextHash = dfl_l1_hash(cv);
+            int32_t candidate = table[nextHash];
+            nextS = s + 2 + ((s - nextEmit) >> 5);
+            if (nextS > sLimit) goto emitRemainder;
+            uint64_t now = dfl_ld64u(in + nextS);
+            table[nextHash] = s + DFL_L1_WINDOW;
+            nextHash = dfl_l1_hash(now);
+            t = candidate - DFL_L1_WINDOW;
+            if (s - t < DFL_L1_MAXOFF && (uint32_t)cv == (uint32_t)dfl_ld64u(in + t)) {
+                table[nextHash] = nextS + DFL_L1_WINDOW;
+                break;
+            }
+            cv = now;
+            s = nextS;
+            nextS++;
+            candidate = table[nextHash];
+            now >>= 8;
+            table[nextHash] = s + DFL_L1_WINDOW;
+            t = candidate - DFL_L1_WINDOW;
+            if (s - t < DFL_L1_MAXOFF && (uint32_t)cv == (uint32_t)dfl_ld64u(in + t)) {
+                table[nextHash] = nextS + DFL_L1_WINDOW;
+                break;
+            }
+            cv = now;
+            s = nextS;
+        }
+        for (;;) {
+            int32_t l = dfl_l1_matchlen(in, s + 4, t + 4, be) + 4;
+            while (t > hs && s > nextEmit && in[t - 1] == in[s - 1]) { s--; t--; l++; }
+            for (int32_t k = nextEmit; k < s; k++) dst.lit(in[k]);
+            dst.match_long(l, (uint32_t)(s - t - 1)); // the inlined AddMatchLong: lengths above 258 split
+            s += l;
+            nextEmit = s;
+            if (nextS >= s) s = nextS + 1;
+            if (s >= sLimit) {
+                if (s + l + 8 < be) table[dfl_l1_hash(dfl_ld64u(in + s))] = s + DFL_L1_WINDOW;
+                goto emitRemainder;
+            }
+            uint64_t x = dfl_ld64u(in + s - 2);
+            const int32_t o = DFL_L1_WINDOW + s - 2;
+            table[dfl_l1_hash(x)] = o;
+            x >>= 16;
+            const uint32_t currHash = dfl_l1_hash(x);
+            const int32_t candidate = table[currHash];
+            table[currHash] = o + 2;
+            t = candidate - DFL_L1_WINDOW;
+            if (s - t > DFL_L1_MAXOFF || (uint32_t)x != (uint32_t)dfl_ld64u(in + t)) { cv = x >> 8; s++; break; }
+        }
+    }
+emitRemainder:
+    if (nextEmit < be && dst.s->n != 0)
+        for (int32_t k = nextEmit; k < be; k++) dst.lit(in[k]);
+}
+
+// An input the BestSpeed lane refuses (B2C_ERR_ARG): over src_stride, or over the cap
+B2C_DEV bool dfl_l1_refused(const DflParams &P, uint32_t i) {
+    return dfl_too_big(P, i) || P.src_sizes[i] > DFL_L1_MAX_INPUT;
+}
+
+// One lane: input i as one member of P.format, written as the reference's writers write it for Writes then Close.  slot:
+// the lane's scratch (a zeroed table of DFL_L1_TABLE entries, DFL_L1_TOKENS tokens, a DflSlot and a DflState).  Result:
+// out_sizes[i] = the member's bytes before its trailer (the check kernel appends it), B2C_ERR_DST_SMALL or B2C_ERR_ARG.
+B2C_DEV void dfl_l1_lane(const DflParams &P, uint32_t i, uint32_t slot, int32_t *table) {
+    if (dfl_l1_refused(P, i)) { P.out_sizes[i] = DFL_ERR_ARG; return; }
+    const int32_t n = (int32_t)P.src_sizes[i];
+    const uint8_t *in = dfl_src(P, i);
+    DflSlot *sl = P.slots + slot;
+    DflTok tok{sl, P.tokens + (size_t)slot * DFL_L1_TOKENS};
+    DflWriter w;
+    w.st = P.state + slot; w.out = dfl_dst(P, i); w.cap = dfl_cap(P, i);
+    w.bits = 0; w.n = 0; w.nbits = 0; w.overflow = false; w.lastHeader = 0; w.lastHuffMan = 0; w.litSel = 0;
+    if (P.format == DFL_FMT_ZLIB) { w.byte(0x78); w.byte(0x01); }   // zlib/writer.go:95-130 at BestSpeed
+    for (uint32_t k = 0; k < P.hlen; k++) w.byte(P.hdr[k]);
+    int32_t hs = 0, hl = 0;                            // e.hist: its start in the input and its length
+    for (int32_t bs = 0; bs < n && !w.overflow;) {     // storeFast (deflate.go:713-751) per window
+        const int32_t len = n - bs < DFL_L1_WINDOW ? n - bs : DFL_L1_WINDOW, be = bs + len;
+        const bool sync = be == n;                     // the window Close stores
+        const uint8_t *blk = in + bs;
+        if (len < 128) {                               // only the last window is ever short
+            if (len <= 32) w.stored(blk, (uint32_t)len, false);
+            else dfl_block_huff<7>(w, false, blk, (uint32_t)len, true);
+            break;
+        }
+        if (hl + len > DFL_L1_HIST && hl > 0) { hs += hl - DFL_L1_MAXOFF; hl = DFL_L1_MAXOFF; }   // addBlock's move
+        hl += len;
+        for (uint32_t k = 0; k < sizeof(DflSlot) / 4; k++) reinterpret_cast<uint32_t *>(sl)[k] = 0;
+        dfl_l1_parse(in, hs, bs, be, tok, table);
+        if (sl->n == 0) w.stored(blk, (uint32_t)len, false);
+        else if ((int)sl->n > len - (len >> 4)) dfl_block_huff<7>(w, false, blk, (uint32_t)len, sync);
+        else dfl_block_dynamic<7>(w, sl, tok.t, false, blk, (uint32_t)len, sync);
+        bs = be;
+    }
+    w.stored_header(0, true);                          // close: writeStoredHeader(0, true), flush
+    w.flush();
+    P.out_sizes[i] = w.overflow ? -4 : (int64_t)w.n;
+}
+
+// One warp: input i's CRC-32 (raw, gzip) or Adler-32 (zlib) to crc_out, and the trailer: gzip CRC-32 and ISIZE
+// (gzip/gzip.go:264-290), zlib the Adler-32 big-endian (zlib/writer.go:170-195).  Raw without crc_out has nothing to do.
+B2C_DEV void dfl_l1_check_warp(const DflParams &P, uint32_t i, const uint32_t *tab, unsigned lane) {
+    if (dfl_l1_refused(P, i) || (P.format == DFL_FMT_RAW && !P.crc_out)) return;
+    const uint32_t n = P.src_sizes[i];
+    const uint8_t *in = dfl_src(P, i);
+    const uint32_t c = P.format == DFL_FMT_ZLIB ? inf_adler32_warp(in, n, lane) : inf_crc32_warp(in, n, tab, lane);
+    if (lane != 0) return;
+    if (P.crc_out) P.crc_out[i] = c;
+    const int64_t r = P.out_sizes[i];
+    if (P.format == DFL_FMT_RAW || r < 0) return;
+    const uint32_t tl = P.format == DFL_FMT_GZIP ? 8 : 4;
+    if ((uint64_t)r + tl > dfl_cap(P, i)) { P.out_sizes[i] = -4; return; }
+    uint8_t *o = dfl_dst(P, i) + r;
+    if (P.format == DFL_FMT_GZIP)
+        for (int k = 0; k < 4; k++) { o[k] = (uint8_t)(c >> (8 * k)); o[4 + k] = (uint8_t)(n >> (8 * k)); }
+    else
+        for (int k = 0; k < 4; k++) o[k] = (uint8_t)(c >> (24 - 8 * k));
+    P.out_sizes[i] = r + tl;
+}
+
 #ifndef B2C_EMU
 constexpr int DFL_PARSE_WARPS = 2, DFL_ENCODE_LANES = 64, DFL_CRC_WARPS = 4;
 extern "C" __global__ void __launch_bounds__(DFL_PARSE_WARPS * 32) b2c_deflate_parse_kernel(DflParams P, uint32_t nchunks) {
@@ -706,6 +880,18 @@ extern "C" __global__ void __launch_bounds__(DFL_CRC_WARPS * 32) b2c_deflate_crc
     __syncthreads();
     const uint32_t i = blockIdx.x * DFL_CRC_WARPS + (threadIdx.x >> 5);
     if (i < nchunks) dfl_crc_warp(P, i, tab, threadIdx.x & 31);
+}
+// BestSpeed: lane i - i0 of a pass takes input i with the pass's scratch slot i - i0; tables: the pass's zeroed tables
+extern "C" __global__ void __launch_bounds__(DFL_ENCODE_LANES) b2c_deflate_l1_kernel(DflParams P, int32_t *tables, uint32_t i0, uint32_t i1) {
+    const uint32_t i = i0 + blockIdx.x * DFL_ENCODE_LANES + threadIdx.x;
+    if (i < i1) dfl_l1_lane(P, i, i - i0, tables + (size_t)(i - i0) * DFL_L1_TABLE);
+}
+extern "C" __global__ void __launch_bounds__(DFL_CRC_WARPS * 32) b2c_deflate_l1_check_kernel(DflParams P, uint32_t nchunks) {
+    __shared__ uint32_t tab[256];
+    inf_crc_table(tab, threadIdx.x, blockDim.x);
+    __syncthreads();
+    const uint32_t i = blockIdx.x * DFL_CRC_WARPS + (threadIdx.x >> 5);
+    if (i < nchunks) dfl_l1_check_warp(P, i, tab, threadIdx.x & 31);
 }
 #endif
 

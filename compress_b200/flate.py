@@ -5,6 +5,10 @@ Encoder.encode_chunks / encode_device write flate.StatelessDeflate output (flate
 or as gzip members, byte-identical to the reference: every block of every input is parsed at once on the device.
 StatelessDeflate and NewStatelessWriter are thin layers over one such call.
 
+Encoder.best_speed_chunks / best_speed_device write what flate.NewWriter(w, BestSpeed) -- or zlib / gzip
+.NewWriterLevel(w, BestSpeed) -- writes for Writes then Close, byte-identical to the reference: one lane per input parses
+and writes its windows in order.  NewWriter(w, BestSpeed) buffers its Writes and makes one such call at Close.
+
 Decoder.decode_chunks / decode_device decode a batch of whole streams in one call, one lane per stream; results are the
 content's bytes or the reference's error class (B2C_ERR_* codes, see include/b2c.h).  NewReader and the readers of the gzip
 and zlib modules are thin layers over one such call for a single input: a single stream is serial, so one long stream
@@ -24,6 +28,8 @@ MAX_CAP = (1 << 32) - 1                      # contents are under 4 GiB
 
 
 MAX_STATELESS_DICT = 8 << 10                 # only the last 8 KiB of a dict are used
+BestSpeed = 1
+MAX_BEST_SPEED_INPUT = 1 << 30               # a larger input is B2C_ERR_ARG
 
 
 class CorruptInputError(Exception):
@@ -175,6 +181,55 @@ class Encoder(Context):
         return (*t.results(), [int(c) for c in cout])
 
 
+    def best_speed_device(self, src, src_sizes, src_stride, dst=None, dst_cap=None, out_sizes=None, format=RAW, header=b"",
+                          check_out=None, src_offsets=None):
+        """Device-resident batch at BestSpeed: input i is src_sizes[i] bytes at src + i * src_stride (or src +
+        src_offsets[i], each at most src_stride bytes), written as one member of `format` (RAW, ZLIB, or GZIP with this
+        member header) into row i of dst ([n, dst_cap] uint8).  check_out: optional int32 tensor for each input's CRC-32
+        (RAW, GZIP) or Adler-32 (ZLIB).  Asynchronous on the current stream.  Returns (dst, out_sizes): out_sizes[i] =
+        bytes or a negative B2C_ERR_* code."""
+        assert src.is_cuda and src.dtype == torch.uint8
+        n = src_sizes.numel()
+        if dst_cap is None:
+            dst_cap = BestSpeedBound(src_stride) + _container_bytes(format, header)
+        if dst is None:
+            dst = torch.empty((n, dst_cap), dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty((n,), dtype=torch.int64, device=src.device)
+        stream = torch.cuda.current_stream(src.device).cuda_stream
+        check(lib.b2c_flate_best_speed_device(self._ctx, format, 0, src.data_ptr(), src_stride,
+                                              None if src_offsets is None else src_offsets.data_ptr(), src_sizes.data_ptr(),
+                                              bytes(header), len(header), dst.data_ptr(),
+                                              dst.shape[1] if dst.dim() == 2 else dst_cap, None, dst_cap,
+                                              out_sizes.data_ptr(), None if check_out is None else check_out.data_ptr(), n,
+                                              ctypes.c_void_p(stream)), self._ctx)
+        return dst, out_sizes
+
+    def best_speed_chunks(self, inputs, format=RAW, header=b"", caps=None):
+        """Host buffers at BestSpeed: one member of `format` per input.  Returns (outputs, codes, checks): outputs[i] the
+        bytes (None on error), codes[i] their length or a negative B2C_ERR_* code, checks[i] the CRC-32 (RAW, GZIP) or
+        Adler-32 (ZLIB) of input i."""
+        n = len(inputs)
+        if n == 0:
+            return [], [], []
+        if caps is None:
+            caps = [BestSpeedBound(len(b)) + _container_bytes(format, header) for b in inputs]
+        t = PointerTable(inputs, caps)
+        chk = (ctypes.c_uint32 * n)()
+        check(lib.b2c_flate_best_speed_chunks(self._ctx, format, 0, t.srcs, t.ssz, bytes(header), len(header), t.dsts,
+                                              t.dcap, t.res, chk, n), self._ctx)
+        return (*t.results(), [int(c) for c in chk])
+
+
+def BestSpeedBound(n):
+    """The largest raw output of an n-byte input at BestSpeed (a zlib stream adds 6 bytes, a gzip member its header + 8)."""
+    return int(lib.b2c_flate_best_speed_bound(n))
+
+
+def _container_bytes(format, header):
+    return 6 if format == ZLIB else (len(header) + 8 if format == GZIP else 0)
+
+
 _enc = None
 
 
@@ -221,3 +276,64 @@ class _StatelessWriter:
 
 def NewStatelessWriter(dst):
     return _StatelessWriter(dst)
+
+
+def best_speed_member(data, format, header=b""):
+    """One member of `format` at BestSpeed for the bytes of all Writes, encoded in one device call; raises on error."""
+    outs, codes, _ = _encoder().best_speed_chunks([data], format, header)
+    if codes[0] < 0:
+        raise B2CError(f"libb200comp error {codes[0]}: {lib.b2c_strerror(codes[0]).decode()}")
+    return outs[0]
+
+
+class BufferedWriter:
+    """The Write / Close side of a writer at BestSpeed: Writes are buffered and Close encodes them in one device call --
+    without Flush the reference's blocks depend on the byte count alone, so the Writes' boundaries do not matter.  Flush
+    (a sync flush) is not built.  Subclasses give _member(data)."""
+
+    def __init__(self, w):
+        self.Reset(w)
+
+    def Reset(self, w):
+        """Discards the buffered bytes; the next Write starts a new member on w."""
+        self._w, self._buf, self._closed = w, bytearray(), False
+
+    def Write(self, p):
+        if self._closed:
+            raise ValueError("write after Close")
+        p = bytes(p)
+        if len(self._buf) + len(p) > MAX_BEST_SPEED_INPUT:
+            raise ValueError("the device encodes at most 1 GiB per member at BestSpeed")
+        self._buf += p
+        return len(p)
+
+    write = Write
+
+    def Flush(self):
+        raise NotImplementedError("Flush (a sync flush) is not built on the device at BestSpeed; Close ends the member")
+
+    def Close(self):
+        if self._closed:
+            return
+        self._closed = True
+        self._w.write(self._member(bytes(self._buf)))
+        self._buf = bytearray()
+
+    close = Close
+
+
+class Writer(BufferedWriter):
+    """flate.Writer at BestSpeed (flate/deflate.go): a raw DEFLATE stream, encoded on the device at Close."""
+
+    def __init__(self, w, level=BestSpeed):
+        if level != BestSpeed:
+            raise ValueError("flate: only BestSpeed (1) is built on the device for NewWriter; level %r is not" % (level,))
+        super().__init__(w)
+
+    def _member(self, data):
+        return best_speed_member(data, RAW)
+
+
+def NewWriter(w, level):
+    """flate.NewWriter; only BestSpeed is built."""
+    return Writer(w, level)

@@ -2,7 +2,8 @@
 input is serial; see flate.Decoder for batches).  The first member's Header is parsed on the host.
 
 gzip.NewWriterLevel(w, StatelessCompression) (gzip/gzip.go): a Writer whose every Write is one device call of
-flate.StatelessDeflate; the CRC-32 is continued on the device.  Other levels are not built."""
+flate.StatelessDeflate; the CRC-32 is continued on the device.  gzip.NewWriterLevel(w, BestSpeed): a Writer that buffers its
+Writes and encodes the member in one device call at Close.  Other levels are not built."""
 import io
 import struct
 from dataclasses import dataclass
@@ -12,6 +13,7 @@ from .flate import ErrUnexpectedEOF  # noqa: F401
 
 
 StatelessCompression = -3
+BestSpeed, BestCompression = 1, 9
 # time.Time{}.Unix(): the reference writes uint32(ModTime.Unix()) without a zero check, so an unset ModTime is this
 ZERO_MODTIME = -62135596800
 
@@ -99,24 +101,30 @@ def NewReader(r):
 
 
 class Writer:
-    """gzip.Writer at StatelessCompression: Name / Comment / Extra / ModTime (Unix seconds; unset is Go's zero time) / OS
-    set before the first
-    Write go into the header; each Write(p) is StatelessDeflate(p, false), Close writes StatelessDeflate(nil, true), the
-    CRC-32 and ISIZE.  Flush writes nothing (the stateless writer keeps no pending data)."""
+    """gzip.Writer at StatelessCompression or BestSpeed: Name / Comment / Extra / ModTime (Unix seconds; unset is Go's
+    zero time) / OS set before the first Write (at BestSpeed: before Close) go into the header.
+    StatelessCompression: each Write(p) is StatelessDeflate(p, false), Close writes StatelessDeflate(nil, true), the
+    CRC-32 and ISIZE; Flush writes nothing (the stateless writer keeps no pending data).
+    BestSpeed: the Writes are buffered and Close writes the whole member (header with XFL 4, the stream, CRC-32 and ISIZE)
+    from one device call; Flush (a sync flush) is not built and raises."""
 
     def __init__(self, w, level=StatelessCompression):
-        if level != StatelessCompression:
-            raise ValueError("gzip: only StatelessCompression (-3) is built on the device; level %r is not" % (level,))
+        if level not in (StatelessCompression, BestSpeed):
+            raise ValueError("gzip: only StatelessCompression (-3) and BestSpeed (1) are built on the device; level %r is "
+                             "not" % (level,))
+        self._level = level
         self.Reset(w)
 
     def Reset(self, w):
         """As the reference's Reset (gzip/gzip.go:98-114): the header fields go back to their zero values too."""
         self.Name, self.Comment, self.Extra, self.ModTime, self.OS = "", "", None, ZERO_MODTIME, 255
         self._w, self._wrote, self._closed, self._crc, self._size = w, False, False, 0, 0
+        self._buf = bytearray()
 
     def _header(self):
         flg = (4 if self.Extra is not None else 0) | (8 if self.Name else 0) | (16 if self.Comment else 0)
-        h = b"\x1f\x8b\x08" + bytes([flg]) + struct.pack("<I", int(self.ModTime) & 0xffffffff) + b"\x00" + bytes([self.OS])
+        xfl = 4 if self._level == BestSpeed else (2 if self._level == BestCompression else 0)   # gzip/gzip.go:193-198
+        h = b"\x1f\x8b\x08" + bytes([flg]) + struct.pack("<I", int(self.ModTime) & 0xffffffff) + bytes([xfl, self.OS])
         if self.Extra is not None:
             h += struct.pack("<H", len(self.Extra)) + bytes(self.Extra)
         if self.Name:
@@ -127,6 +135,13 @@ class Writer:
 
     def Write(self, p):
         p = bytes(p)
+        if self._level == BestSpeed:
+            if self._closed:
+                raise ValueError("write after Close")
+            if len(self._buf) + len(p) > flate.MAX_BEST_SPEED_INPUT:
+                raise ValueError("the device encodes at most 1 GiB per member at BestSpeed")
+            self._buf += p
+            return len(p)
         if not self._wrote:
             self._wrote = True
             self._w.write(self._header())
@@ -141,12 +156,17 @@ class Writer:
     write = Write
 
     def Flush(self):
-        pass
+        if self._level == BestSpeed:
+            raise NotImplementedError("Flush (a sync flush) is not built on the device at BestSpeed; Close ends the member")
 
     def Close(self):
         if self._closed:
             return
         self._closed = True
+        if self._level == BestSpeed:
+            self._w.write(flate.best_speed_member(bytes(self._buf), flate.GZIP, self._header()))
+            self._buf = bytearray()
+            return
         if not self._wrote:
             self.Write(b"")
         self._w.write(b"\x03\x00" + struct.pack("<II", self._crc, self._size))
@@ -155,12 +175,13 @@ class Writer:
 
 
 def NewWriterLevel(w, level):
-    """gzip.NewWriterLevel; only StatelessCompression is built."""
+    """gzip.NewWriterLevel; only StatelessCompression and BestSpeed are built."""
     return Writer(w, level)
 
 
-def header_bytes(Name="", Comment="", Extra=None, ModTime=ZERO_MODTIME, OS=255):
-    """The member header gzip.Writer writes for these fields (XFL 0), as flate.Encoder takes it for format GZIP."""
-    w = Writer(io.BytesIO())
+def header_bytes(Name="", Comment="", Extra=None, ModTime=ZERO_MODTIME, OS=255, level=StatelessCompression):
+    """The member header gzip.Writer writes for these fields at this level (XFL 4 at BestSpeed, else 0), as flate.Encoder
+    takes it for format GZIP."""
+    w = Writer(io.BytesIO(), level)
     w.Name, w.Comment, w.Extra, w.ModTime, w.OS = Name, Comment, Extra, ModTime, OS
     return w._header()

@@ -1,9 +1,14 @@
 """zlib.NewReader on the device (zlib/reader.go): the whole zlib stream is decoded in one device call, on one GPU lane
-(a single stream is serial; see flate.Decoder for batches)."""
+(a single stream is serial; see flate.Decoder for batches).
+
+zlib.NewWriterLevel(w, BestSpeed) (zlib/writer.go): a Writer that buffers its Writes and encodes the stream in one device
+call at Close.  Other levels, and so NewWriter's DefaultCompression, are not built."""
 import io
 
 from . import flate
 from .flate import ErrUnexpectedEOF  # noqa: F401
+
+NoCompression, BestSpeed, BestCompression, DefaultCompression, HuffmanOnly = 0, 1, 9, -1, -2
 
 
 class ErrHeader(Exception):
@@ -23,3 +28,26 @@ def NewReader(r):
     errors are raised here."""
     data = r if isinstance(r, (bytes, bytearray, memoryview)) else r.read()
     return io.BytesIO(flate._decoder().decode_all(bytes(data), flate.ZLIB))
+
+
+class Writer(flate.BufferedWriter):
+    """zlib.Writer at BestSpeed: header 78 01, the DEFLATE stream and the Adler-32, written at Close."""
+
+    def __init__(self, w, level=DefaultCompression):
+        if level != BestSpeed:
+            raise ValueError("zlib: only BestSpeed (1) is built on the device; level %r is not" % (level,))
+        super().__init__(w)
+
+    def _member(self, data):
+        return flate.best_speed_member(data, flate.ZLIB)
+
+
+def NewWriter(w):
+    """zlib.NewWriter: DefaultCompression, which is not built, so this raises ValueError; use NewWriterLevel(w,
+    BestSpeed)."""
+    return Writer(w)
+
+
+def NewWriterLevel(w, level):
+    """zlib.NewWriterLevel; only BestSpeed is built."""
+    return Writer(w, level)

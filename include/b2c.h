@@ -295,6 +295,31 @@ B2C_API int b2c_flate_stateless_chunks(b2c_ctx *ctx, int format, int flags, cons
                                        int64_t *sizes_out, const uint32_t *crc_in, uint32_t *crc_out, size_t n);
 
 /*
+ * DEFLATE at BestSpeed (level 1), byte-identical to the reference on amd64: input i is one member of the given format as
+ * the reference's writers write it for any number of Write(p) calls (together, input i) followed by Close() -- B2C_FLATE_RAW
+ * flate.NewWriter(w, BestSpeed); B2C_FLATE_ZLIB zlib.NewWriterLevel(w, BestSpeed): header 78 01, the stream, Adler-32
+ * big-endian; B2C_FLATE_GZIP gzip.NewWriterLevel(w, BestSpeed): hdr (the member header, >= 10 bytes, XFL 4, built by the
+ * caller and copied into every member), the stream, CRC-32 and ISIZE.  Without Flush the blocks depend on the byte count
+ * alone (65 535-byte windows), so the Writes' boundaries do not matter.  Results: the member's bytes, or
+ * B2C_ERR_DST_SMALL (nothing is written past the destination), or B2C_ERR_ARG for an input over 1 GiB or, in the _device
+ * call, over src_stride; the other inputs are unaffected.  d_check_out / check_out (optional) receive each input's CRC-32
+ * (raw, gzip) or Adler-32 (zlib).  Each member is parsed and written on one lane, in order (each window's matches reach
+ * into the windows before it): throughput comes from batches of many inputs.  The context holds about 385 KiB of scratch
+ * per input in flight, at most 4 GiB (larger batches run in passes).  b2c_flate_best_speed_bound(n): the largest raw
+ * output of an n-byte input (add 6 for zlib, hlen + 8 for gzip).  Argument conventions as b2c_flate_stateless_device /
+ * _chunks; flags is 0.
+ */
+B2C_API size_t b2c_flate_best_speed_bound(size_t n);
+B2C_API int b2c_flate_best_speed_device(b2c_ctx *ctx, int format, int flags, const void *d_src, size_t src_stride,
+                                        const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, const void *hdr,
+                                        size_t hlen, void *d_dst, size_t dst_stride, const uint64_t *d_dst_offsets,
+                                        uint32_t dst_cap, int64_t *d_out_sizes, uint32_t *d_check_out, uint32_t nchunks,
+                                        void *stream);
+B2C_API int b2c_flate_best_speed_chunks(b2c_ctx *ctx, int format, int flags, const void *const *srcs,
+                                        const size_t *src_sizes, const void *hdr, size_t hlen, void *const *dsts,
+                                        const size_t *dst_caps, int64_t *sizes_out, uint32_t *check_out, size_t n);
+
+/*
  * S2 / Snappy STREAMS (the framing format: s2.Writer.EncodeBuffer, s2/writer.go:357-470, and s2.Reader over a buffer,
  * s2/reader.go:249-420; constants and the masked CRC32-C: s2/s2.go:75-126).  A stream = the identifier chunk, then per
  * block (<= 64 KiB here, WriterBlockSize) one chunk: type (0 compressed, 1 uncompressed), 24-bit length, checksum of the

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""Device-resident StatelessDeflate rates (input GB/s) on helpers.synth_text_torch text, raw and as gzip members, in two
-shapes: --gib of text as 64 KiB inputs and as 64 MiB inputs.  Each batch is encoded whole and timed with CUDA events
+"""Device-resident StatelessDeflate and BestSpeed rates (input GB/s) and ratios on helpers.synth_text_torch text, raw and as
+gzip members (BestSpeed also as zlib streams), in two shapes: --gib of text as 64 KiB inputs and as 64 MiB inputs.  Each batch is encoded whole and timed with CUDA events
 (--warmup warm-ups, --steps steps, --big-steps for the 64 MiB shape; --shapes / --formats pick rows, so that the rows
 can be split across runs); the
-parse / encode / crc kernels are timed with torch.profiler in a run of their own.  The device inflate of the raw output
+parse / encode / crc (BestSpeed: l1 / l1_check) kernels are timed with torch.profiler in a run of their own.  The device inflate of the raw output
 is timed in the same session, and zlib.compress at level 1 on every host core over the same inputs is a CPU line for
 context (it is zlib's level 1, not the reference's StatelessDeflate, which is Go and does not run here).  Records the card's
 name and power limit.  Prints one JSON line (and writes it to --out).
 usage: deflate_times.py [--gib G] [--warmup W] [--steps K] [--big-steps K] [--big-mib M] [--shapes small,big]
-       [--formats raw,gzip] [--no-inflate] [--out FILE]"""
+       [--formats raw,zlib,gzip] [--levels stateless,best_speed] [--no-inflate] [--out FILE]"""
 import argparse
 import json
 import os
@@ -27,7 +27,9 @@ import helpers as H
 from compress_b200 import flate
 
 KERNELS = ["b2c_deflate_parse_kernel", "b2c_deflate_encode_kernel", "b2c_deflate_crc_kernel"]
+KERNELS_L1 = ["b2c_deflate_l1_kernel", "b2c_deflate_l1_check_kernel"]
 HDR = b"\x1f\x8b\x08\x00\x00\x00\x00\x00\x00\xff"
+HDR_L1 = b"\x1f\x8b\x08\x00\x00\x09\x6e\x88\x04\xff"    # XFL 4, as gzip.NewWriterLevel(w, BestSpeed) writes it
 
 
 def timed(fn, warmup, steps):
@@ -48,14 +50,14 @@ def timed(fn, warmup, steps):
     return total / steps
 
 
-def kernel_ms(fn):
+def kernel_ms(fn, kernels=KERNELS):
     from torch.profiler import profile, ProfilerActivity
     fn()
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
         torch.cuda.synchronize()
-    out = {k: 0.0 for k in KERNELS}
+    out = {k: 0.0 for k in kernels}
     for e in prof.key_averages():
         if e.key in out:
             out[e.key] = round(e.device_time_total / 1000.0, 3)
@@ -70,7 +72,8 @@ def main():
     ap.add_argument("--big-steps", type=int, default=20)
     ap.add_argument("--big-mib", type=int, default=64)
     ap.add_argument("--shapes", default="small,big", help="small: 64 KiB inputs, big: --big-mib inputs")
-    ap.add_argument("--formats", default="raw,gzip")
+    ap.add_argument("--formats", default="raw,zlib,gzip", help="zlib: BestSpeed rows only")
+    ap.add_argument("--levels", default="stateless,best_speed")
     ap.add_argument("--no-inflate", action="store_true", help="skip the device inflate of the raw output")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -89,7 +92,7 @@ def main():
         dst = torch.empty((n, cap), dtype=torch.uint8, device=dev)
         out = torch.empty((n,), dtype=torch.int64, device=dev)
         for fmt, name, hdr in ((flate.RAW, "raw", b""), (flate.GZIP, "gzip", HDR)):
-            if name not in a.formats:
+            if name not in a.formats or "stateless" not in a.levels:
                 continue
             call = lambda: enc.encode_device(src, sizes, piece, dst=dst, dst_cap=cap, out_sizes=out, format=fmt, header=hdr)  # noqa: E731
             ms = timed(call, warm, steps)
@@ -111,6 +114,23 @@ def main():
                 assert bool((dsz == piece).all()) and bool((back.reshape(-1) == src[:n * piece]).all())
                 row["inflate_ms"] = round(dms, 3)
                 row["inflate_output_GBps"] = round(total / dms / 1e6, 2)
+            res["rows"].append(row)
+            print(json.dumps(row), flush=True)
+        del dst
+        if "best_speed" not in a.levels:
+            continue
+        cap = flate.BestSpeedBound(piece) + len(HDR_L1) + 8
+        dst = torch.empty((n, cap), dtype=torch.uint8, device=dev)
+        for fmt, name, hdr in ((flate.RAW, "raw", b""), (flate.ZLIB, "zlib", b""), (flate.GZIP, "gzip", HDR_L1)):
+            if name not in a.formats:
+                continue
+            call = lambda: enc.best_speed_device(src, sizes, piece, dst=dst, dst_cap=cap, out_sizes=out, format=fmt, header=hdr)  # noqa: E731
+            ms = timed(call, warm, steps)
+            o = out.cpu()
+            assert int(o.min()) > 0
+            row = {"shape": "%d x %d KiB" % (n, piece >> 10), "level": "best_speed", "format": name, "ms": round(ms, 3),
+                   "input_GBps": round(total / ms / 1e6, 2), "ratio": round(total / int(o.sum()), 4), "steps": steps,
+                   "kernel_ms": kernel_ms(call, KERNELS_L1)}
             res["rows"].append(row)
             print(json.dumps(row), flush=True)
         del dst
