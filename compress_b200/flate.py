@@ -43,6 +43,11 @@ class ErrUnexpectedEOF(EOFError):
 class Decoder(Context):
     """Batches of raw DEFLATE / zlib / gzip streams decoded on one GPU."""
 
+    @property
+    def launches(self):
+        """Kernel launches on this context so far: a decode call launches 3 per pass over its record scratch."""
+        return int(lib.b2c_launch_count(self._ctx))
+
     def decode_device(self, src, src_sizes, src_stride, dst=None, dst_cap=1 << 16, out_sizes=None, format=GZIP,
                       multistream=True, src_offsets=None):
         """Device-resident batch: input i is src_sizes[i] bytes at src + i * src_stride (or src + src_offsets[i], each at
