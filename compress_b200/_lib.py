@@ -151,6 +151,16 @@ def _load():
     lib.b2c_flate_best_speed_chunks.argtypes = [
         c.c_void_p, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_char_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p,
         c.c_void_p, c.c_size_t]
+    lib.b2c_flate_nolz_bound.restype = c.c_size_t
+    lib.b2c_flate_nolz_bound.argtypes = [c.c_int, c.c_size_t]
+    lib.b2c_flate_nolz_device.restype = c.c_int
+    lib.b2c_flate_nolz_device.argtypes = [
+        c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_char_p, c.c_size_t,
+        c.c_void_p, c.c_size_t, c.c_void_p, c.c_uint32, c.c_void_p, c.c_void_p, c.c_uint32, c.c_void_p]
+    lib.b2c_flate_nolz_chunks.restype = c.c_int
+    lib.b2c_flate_nolz_chunks.argtypes = [
+        c.c_void_p, c.c_int, c.c_int, c.c_int, c.c_void_p, c.c_void_p, c.c_char_p, c.c_size_t, c.c_void_p, c.c_void_p,
+        c.c_void_p, c.c_void_p, c.c_size_t]
     lib.b2c_huf_compress_device.restype = c.c_int
     lib.b2c_huf_compress_device.argtypes = [
         c.c_void_p, c.c_int, c.c_void_p, c.c_size_t, c.c_void_p, c.c_uint32, c.c_void_p, c.c_size_t, c.c_void_p,
@@ -198,6 +208,7 @@ EXPORTED_SYMBOLS = [
     "b2c_flate_decode_device", "b2c_flate_decode_chunks",
     "b2c_flate_stateless_bound", "b2c_flate_stateless_device", "b2c_flate_stateless_chunks",
     "b2c_flate_best_speed_bound", "b2c_flate_best_speed_device", "b2c_flate_best_speed_chunks",
+    "b2c_flate_nolz_bound", "b2c_flate_nolz_device", "b2c_flate_nolz_chunks",
 ]
 
 

@@ -2053,6 +2053,98 @@ int b2c_flate_best_speed_chunks(b2c_ctx *ctx, int format, int flags, const void 
     return B.scatter(dsts, sizes_out, dst_caps);
 }
 
+// ---- HuffmanOnly / NoCompression: flate.NewWriter(w, -2 | 0), zlib / gzip.NewWriterLevel(w, -2 | 0) -----------------
+// Window slot = input * max_windows + k (max_windows from src_stride, or from the largest input of a _chunks call), one
+// DflNolzWin record each in d_dfl; a batch whose records need more than kDflNolzPassBytes runs in passes over whole
+// inputs (an input of under 4 GiB has at most 131 072 windows, 230 MiB of records).
+static const uint64_t kDflNolzPassBytes = (uint64_t)4 << 30;
+// The bound.  Every window is one block.
+//  - Level 0: stored blocks, len + 5 bytes each, then Close's 03 00.
+//  - Level -2, stored: up to 15 bits of the EOB the block before owed, the 3-bit header and its byte's end, LEN / NLEN:
+//    len + 7 bytes.
+//  - Level -2, Huffman: chosen only when estBits, which counts the window's codes under its own table (EOB included) or
+//    the reused table's codes, is below the stored size (len + 5) * 8.  A reused table adds its EOB and the owed EOB: 30
+//    bits.  A new table adds the owed EOB and a real header of at most 17 + 19 * 3 + 258 * 7 = 1 880 bits; estBits guessed
+//    560 bits for it when no table was in force, but only lastHeader -- a header that can be much shorter -- when it
+//    replaces one, so the block can exceed the stored size by up to 1 894 bits, not only 1 320: len + 242 bytes.
+// Close adds 10 bits and the last partial byte: 2 bytes.  zlib adds 6 bytes, gzip hlen + 8.
+size_t b2c_flate_nolz_bound(int level, size_t n) {
+    if (level == 0) return n + 5 * (n / DFL_NOLZ_WINDOW_STORE + 1) + 2;
+    if (level == -2) return n + 242 * (n / DFL_NOLZ_WINDOW_HUFF + 1) + 2;
+    return 0;
+}
+
+static int launch_nolz(b2c_ctx *ctx, DflNolzParams P, uint32_t n, const void *hdr, size_t hlen, cudaStream_t st) {
+    const uint64_t per = (uint64_t)P.max_windows * sizeof(DflNolzWin), fit = kDflNolzPassBytes / per;
+    const uint32_t inputs = fit >= n ? n : (fit ? (uint32_t)fit : 1);
+    Layout L;
+    const size_t oWin = L.take((size_t)inputs * per), oHdr = L.take(hlen ? hlen : 1);
+    { int r = reserve(ctx, ctx->d_dfl, L.end); if (r) return r; }
+    { int r = ctx_order_begin(ctx, st); if (r) return r; }
+    P.wins = ctx->d_dfl.at<DflNolzWin>(oWin);
+    P.hdr = ctx->d_dfl.p + oHdr; P.hlen = (uint32_t)hlen;
+    if (hlen) CK(cudaMemcpyAsync(ctx->d_dfl.p + oHdr, hdr, hlen, cudaMemcpyHostToDevice, st));
+    const bool analyse = P.level != 0 || P.format != B2C_FLATE_RAW || P.crc_out;
+    for (uint32_t i0 = 0; i0 < n; i0 += inputs) {
+        P.i0 = i0; P.i1 = n - i0 < inputs ? n : i0 + inputs;
+        const uint64_t slots = (uint64_t)(P.i1 - P.i0) * P.max_windows;
+        if (analyse) b2c_deflate_nolz_analyse_kernel<<<(unsigned)slots, DFL_NOLZ_THREADS, 0, st>>>(P);
+        b2c_deflate_nolz_plan_kernel<<<(P.i1 - P.i0 + DFL_NOLZ_PLAN_WARPS - 1) / DFL_NOLZ_PLAN_WARPS, DFL_NOLZ_PLAN_WARPS * 32, 0, st>>>(P);
+        b2c_deflate_nolz_emit_kernel<<<(unsigned)slots, DFL_NOLZ_THREADS, 0, st>>>(P);
+        ctx->launches += analyse ? 3 : 2;
+        if (P.level != 0) {                            // level 0 is byte-aligned: no byte is shared
+            b2c_deflate_nolz_finish_kernel<<<(unsigned)((slots + DFL_NOLZ_THREADS - 1) / DFL_NOLZ_THREADS), DFL_NOLZ_THREADS, 0, st>>>(P, slots);
+            ctx->launches += 1;
+        }
+        CK(cudaGetLastError());
+    }
+    return ctx_order_end(ctx, st);
+}
+
+int b2c_flate_nolz_device(b2c_ctx *ctx, int level, int format, int flags, const void *d_src, size_t src_stride,
+                          const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, const void *hdr, size_t hlen,
+                          void *d_dst, size_t dst_stride, const uint64_t *d_dst_offsets, uint32_t dst_cap,
+                          int64_t *d_out_sizes, uint32_t *d_check_out, uint32_t nchunks, void *stream) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if ((level != 0 && level != -2) || !best_speed_args_ok(format, flags, hdr, hlen)) return B2C_ERR_ARG;
+    if (!d_src_sizes || !d_out_sizes || src_stride == 0 || src_stride > 0xffffffffull) return B2C_ERR_ARG;
+    if (nchunks == 0) return B2C_OK;
+    CK(cudaSetDevice(ctx->device));
+    DflNolzParams P;
+    memset(&P, 0, sizeof(P));
+    P.src_base = (const uint8_t *)d_src; P.src_stride = src_stride; P.src_offsets = d_src_offsets; P.src_sizes = d_src_sizes;
+    P.dst_base = (uint8_t *)d_dst; P.dst_stride = dst_stride; P.dst_offsets = d_dst_offsets; P.dst_cap = dst_cap;
+    P.out_sizes = d_out_sizes; P.crc_out = d_check_out;
+    P.format = format; P.level = level;
+    P.max_windows = dfl_nolz_windows(src_stride, level);
+    return launch_nolz(ctx, P, nchunks, hdr, hlen, (cudaStream_t)stream);
+}
+
+int b2c_flate_nolz_chunks(b2c_ctx *ctx, int level, int format, int flags, const void *const *srcs, const size_t *src_sizes,
+                          const void *hdr, size_t hlen, void *const *dsts, const size_t *dst_caps, int64_t *sizes_out,
+                          uint32_t *check_out, size_t n) {
+    if (!ctx) return B2C_ERR_NO_DEVICE;
+    if ((level != 0 && level != -2) || !best_speed_args_ok(format, flags, hdr, hlen)) return B2C_ERR_ARG;
+    if (n == 0) return B2C_OK;
+    int rc = HostBatch::check(ctx, n, src_sizes, 0xffffffffull);
+    if (rc) return rc;
+    HostBatch B(ctx, n, n, {n * 4});                                  // + the checksums
+    B.place_items(src_sizes, 0, dst_caps, 0);
+    uint32_t mw = 1;
+    for (size_t i = 0; i < n; i++) {
+        const uint32_t w = dfl_nolz_windows(src_sizes[i], level);
+        if (w > mw) mw = w;
+    }
+    if ((rc = B.stage_in(srcs, src_sizes))) return rc;
+    DflNolzParams P = B.params<DflNolzParams>();
+    P.crc_out = B.d_at<uint32_t>(B.ex[0]);
+    P.format = format; P.level = level; P.max_windows = mw;
+    if ((rc = launch_nolz(ctx, P, (uint32_t)n, hdr, hlen, ctx->stream))) return rc;
+    if (check_out) CK(cudaMemcpyAsync(check_out, P.crc_out, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = B.results(sizes_out))) return rc;
+    return B.scatter(dsts, sizes_out, dst_caps);
+}
+
 // ---- standalone huff0 blocks ------------------------------------------------------------------------
 int b2c_huf_compress_device(b2c_ctx *ctx, int flags, const void *d_src, size_t src_stride, const uint32_t *d_sizes,
                             uint32_t size_all, void *d_dst, size_t dst_stride, int64_t *d_out_sizes, uint32_t nchunks,

@@ -575,6 +575,20 @@ B2C_DEV void dfl_block_dynamic(DflWriter &w, const DflSlot *s, const uint32_t *t
     w.tokens(toks, s->n, [lc](uint32_t c) { return lc[c]; }, [oc](uint32_t c) { return oc[c]; }, sync);
 }
 
+// writeBlockHuff's quick check for incompressible content (huffman_bit_writer.go:1011-1030), float64 in its order, for
+// the HuffmanOnly analysis.  dfl_block_huff keeps its own copy inline: calling this from it reorders the code of the
+// kernels that use it.
+B2C_DEV bool dfl_huff_incompressible(const uint16_t *lf, uint32_t inlen) {
+    double abs = 0;
+    const double avg = __ddiv_rn((double)inlen, 256.0), max = (double)(inlen * 2);
+    for (int i = 0; i < 256; i++) {
+        const double diff = __dsub_rn((double)lf[i], avg);
+        abs = __dadd_rn(abs, __dmul_rn(diff, diff));
+        if (abs > max) break;
+    }
+    return abs < max;
+}
+
 // writeBlockHuff (huffman_bit_writer.go:987-1174); huffOffset is one code of length 1 for offset 0; PEN as above
 template <int PEN>
 B2C_DEV void dfl_block_huff(DflWriter &w, bool eof, const uint8_t *input, uint32_t inlen, bool sync) {
@@ -863,6 +877,377 @@ B2C_DEV void dfl_l1_check_warp(const DflParams &P, uint32_t i, const uint32_t *t
     P.out_sizes[i] = r + tl;
 }
 
+// ---- HuffmanOnly (-2, ConstantCompression) and NoCompression (0): flate.NewWriter(w, level) for Writes then Close
+// (deflate.go:683-708, :755-827, :865-880), raw or inside the zlib / gzip writers' framing, every window in parallel.
+// Neither level has a match finder.  The compressor fills a window (32 768 bytes at -2, 65 535 at 0) and writes it as one
+// block each time it is full and more bytes arrive; Close writes the last one with sync, then writeStoredHeader(0, true).
+// Without Flush the windows depend on the byte count alone, and all one window passes to the next is the bit writer's
+// table reuse: lastHeader and the table in force.  So the work splits into four passes over a batch:
+//   analysis: one CTA per window: its histogram (shared-memory atomics), its checksum term, writeBlockHuff's float64
+//             test, its own table (generate over 257 symbols) with that table's canReuseBits and dynamic header.
+//   plan:     one warp per input walks its windows in order through writeBlockHuff's reuse decisions -- the reuse cost is
+//             a warp dot product -- and records each window's outcome, owed EOB and bit range; then it sums the member's
+//             size and, if it fits, writes the header, the close block and the trailer.  Level 0 stores every window:
+//             the ranges are closed-form and no walk runs.
+//   emit:     one CTA per window writes the bytes its bit range covers whole; the partial first and last bytes it
+//             shares with its neighbours go to its record.
+//   finish:   one thread per window writes the byte in which its range ends, from the pieces of every range in it.
+// Every output byte is written by one thread, and nothing at all for an input whose member does not fit its capacity.
+constexpr uint32_t DFL_NOLZ_WINDOW_HUFF = 32768, DFL_NOLZ_WINDOW_STORE = 65535;
+constexpr int DFL_NOLZ_PEN = 10;                       // logNewTablePenalty of ConstantCompression
+constexpr uint32_t DFL_NOLZ_STORED = 0xffffffffu;
+constexpr int DFL_NOLZ_THREADS = 256;
+// A Huffman window's bits: the owed EOB (<= 15), then a new table's header (<= 17 + 19 * 3 + 258 * 7 = 1 880) and
+// canReuseBits of its own table, EOB included, or the reused table's codes and EOB.  Both code parts are below the stored
+// size (len + 5) * 8 <= 262 184 (estBits counts them and is below it), so with the 7-bit offset of the first bit the
+// staging holds at most 7 + 15 + 1 880 + 262 183 bits: 8 253 words.
+constexpr uint32_t DFL_NOLZ_STAGE_WORDS = 8256;
+
+struct DflNolzWin {                                    // one window's record (slot = pass input * max_windows + k)
+    uint32_t check[2];                                 // analysis: its checksum term (dfl_nolz_analyse)
+    int32_t est, hdr;                                  // analysis: own table's canReuseBits (-1: stored by the float64
+                                                       // test) and its header's bits
+    uint64_t bit, end;                                 // plan: its bit range in the stream
+    uint32_t eob, use;                                 // plan: the EOB code it owes first (0: none); DFL_NOLZ_STORED
+                                                       // or the window whose table codes its bytes
+    uint32_t sync, pieces;                             // plan: it is the last window; emit: its partial first byte |
+                                                       // its partial last byte << 8
+    uint16_t hist[256];
+    uint32_t codes[260];                               // own table, 257 codes
+    uint8_t hbits[240];                                // own table's dynamic header, LSB first, zero after its bits
+};
+
+struct DflNolzParams {
+    const uint8_t *src_base; size_t src_stride; const uint64_t *src_offsets; const uint32_t *src_sizes;
+    uint8_t *dst_base; size_t dst_stride; const uint64_t *dst_offsets; uint32_t dst_cap; const uint32_t *dst_caps;
+    int64_t *out_sizes; uint32_t *crc_out;
+    const uint8_t *hdr; uint32_t hlen;
+    int format, level;
+    uint32_t max_windows, i0, i1;                      // the inputs of this pass
+    DflNolzWin *wins;                                  // the pass's records
+};
+
+__host__ __device__ inline uint32_t dfl_nolz_window(int level) {
+    return level == 0 ? DFL_NOLZ_WINDOW_STORE : DFL_NOLZ_WINDOW_HUFF;
+}
+__host__ __device__ inline uint32_t dfl_nolz_windows(uint64_t n, int level) {
+    return (uint32_t)((n + dfl_nolz_window(level) - 1) / dfl_nolz_window(level));
+}
+B2C_DEV const uint8_t *dfl_nolz_src(const DflNolzParams &P, uint32_t i) {
+    return P.src_base + (P.src_offsets ? P.src_offsets[i] : (uint64_t)i * P.src_stride);
+}
+B2C_DEV uint8_t *dfl_nolz_dst(const DflNolzParams &P, uint32_t i) {
+    return P.dst_base + (P.dst_offsets ? P.dst_offsets[i] : (uint64_t)i * P.dst_stride);
+}
+// the stream's first byte in the member: after 78 01 (zlib) or the gzip header
+B2C_DEV uint32_t dfl_nolz_hoff(const DflNolzParams &P) {
+    return P.format == DFL_FMT_ZLIB ? 2 : (P.format == DFL_FMT_GZIP ? P.hlen : 0);
+}
+B2C_DEV bool dfl_nolz_refused(const DflNolzParams &P, uint32_t i) { return P.src_stride && P.src_sizes[i] > P.src_stride; }
+B2C_DEV bool dfl_nolz_checked(const DflNolzParams &P) { return P.format != DFL_FMT_RAW || P.crc_out; }
+
+// Slot g of the pass: input i, window k of nw; false for a slot past the input's windows or of a refused input
+struct DflNolzSlot { uint32_t i, k, n, nw; };
+B2C_DEV bool dfl_nolz_slot(const DflNolzParams &P, uint64_t g, DflNolzSlot &s) {
+    s.i = P.i0 + (uint32_t)(g / P.max_windows); s.k = (uint32_t)(g % P.max_windows);
+    if (s.i >= P.i1 || dfl_nolz_refused(P, s.i)) return false;
+    s.n = P.src_sizes[s.i]; s.nw = dfl_nolz_windows(s.n, P.level);
+    return s.k < s.nw;
+}
+
+// The checksum of an input of n bytes is a sum of terms, one per piece [a, b) of it, so the pieces are independent:
+//  - CRC-32: crc(A || B) = crc(A) * x^(8|B|) ^ crc(B) (mod P), so crc = XOR over the pieces of crc(piece) * x^(8 (n - b)).
+//  - Adler-32 with s1 = 1 + the bytes, s2 = the sum of the running s1: s1 = 1 + sum of the pieces' byte sums a, and
+//    s2 = n + sum of (the piece's own s2 from zero) + (n - b) * a.  A term is (a, that s2 part) mod 65 521.
+constexpr uint32_t DFL_ADLER_MOD = 65521;
+B2C_DEV void dfl_nolz_check_term(const DflNolzParams &P, const uint8_t *p, uint32_t len, uint32_t after, const uint32_t *tab,
+                                 unsigned lane, uint32_t *t) {
+    if (P.format == DFL_FMT_ZLIB) {
+        const uint32_t v = inf_adler32_warp(p, len, lane);
+        const uint32_t a = ((v & 0xffff) + DFL_ADLER_MOD - 1) % DFL_ADLER_MOD;
+        const uint32_t b = ((v >> 16) + DFL_ADLER_MOD - len % DFL_ADLER_MOD) % DFL_ADLER_MOD;
+        t[0] = a;
+        t[1] = (uint32_t)(((uint64_t)(after % DFL_ADLER_MOD) * a + b) % DFL_ADLER_MOD);
+    } else {
+        const uint32_t c = inf_crc32_warp(p, len, tab, lane);
+        t[0] = c ? inf_crc_multmodp(inf_crc_xpow8(after), c) : 0;
+        t[1] = 0;
+    }
+}
+B2C_DEV void dfl_nolz_check_add(const DflNolzParams &P, uint32_t *acc, const uint32_t *t) {
+    if (P.format == DFL_FMT_ZLIB) {
+        acc[0] = (acc[0] + t[0]) % DFL_ADLER_MOD;
+        acc[1] = (acc[1] + t[1]) % DFL_ADLER_MOD;
+    } else {
+        acc[0] ^= t[0];
+    }
+}
+
+// analysis: one CTA of DFL_NOLZ_THREADS per window slot g.  Shared: st (a writer state for generate / the header),
+// hist[256], terms[2 * DFL_NOLZ_THREADS / 32], tab (the CRC-32 table).  Level 0 needs the checksum term only.
+B2C_DEV void dfl_nolz_analyse(const DflNolzParams &P, uint64_t g, DflState *st, uint32_t *hist, uint32_t *terms,
+                              const uint32_t *tab, unsigned tid) {
+    DflNolzSlot s;
+    if (!dfl_nolz_slot(P, g, s)) return;
+    const uint32_t W = dfl_nolz_window(P.level), ws = s.k * W, len = s.n - ws < W ? s.n - ws : W;
+    const uint8_t *in = dfl_nolz_src(P, s.i) + ws;
+    DflNolzWin *r = P.wins + g;
+    const bool huff = P.level != 0;
+    if (huff) for (uint32_t t = tid; t < 256; t += DFL_NOLZ_THREADS) hist[t] = 0;
+    __syncthreads();
+    if (huff) for (uint32_t b = tid; b < len; b += DFL_NOLZ_THREADS) atomicAdd(&hist[in[b]], 1u);
+    if (dfl_nolz_checked(P)) {                         // each warp one eighth of the window
+        constexpr uint32_t NWARP = DFL_NOLZ_THREADS / 32;
+        const uint32_t w = tid >> 5, sub = (len + NWARP - 1) / NWARP;
+        const uint32_t lo = w * sub < len ? w * sub : len, hi = lo + sub < len ? lo + sub : len;
+        uint32_t t[2];
+        dfl_nolz_check_term(P, in + lo, hi - lo, s.n - ws - hi, tab, tid & 31, t);
+        if ((tid & 31) == 0) { terms[2 * w] = t[0]; terms[2 * w + 1] = t[1]; }
+        __syncthreads();
+        if (tid == 0) {
+            uint32_t acc[2] = {0, 0};
+            for (uint32_t k = 0; k < NWARP; k++) dfl_nolz_check_add(P, acc, terms + 2 * k);
+            r->check[0] = acc[0]; r->check[1] = acc[1];
+        }
+    }
+    if (!huff) return;
+    __syncthreads();
+    uint16_t *lf = st->literalFreq;
+    for (uint32_t t = tid; t < 256; t += DFL_NOLZ_THREADS) { lf[t] = (uint16_t)hist[t]; r->hist[t] = (uint16_t)hist[t]; }
+    __syncthreads();
+    if (tid == 0) {                                    // writeBlockHuff's per-window part (window <= 32 768: storable)
+        if (len > 1024 && dfl_huff_incompressible(lf, len)) {
+            r->est = -1; r->hdr = 0;
+        } else {
+            lf[DFL_EOB] = 1;
+            dfl_generate(&st->lit[0], lf, DFL_EOB + 1, 15);
+            r->est = dfl_reuse_bits(st->lit[0].codes, lf, DFL_EOB + 1);
+            DflWriter w;
+            w.st = st; w.out = r->hbits; w.cap = sizeof(r->hbits);
+            w.bits = 0; w.n = 0; w.nbits = 0; w.overflow = false; w.lastHeader = 0; w.lastHuffMan = 0; w.litSel = 0;
+            const uint32_t huffOff[1] = {dfl_hcode(0, 1)};
+            w.gen_codegen(DFL_EOB + 1, 1, st->lit[0].codes, huffOff);
+            dfl_generate(&st->cg, st->codegenFreq, DFL_CG, 7);
+            r->hdr = w.header_size();
+            w.dynamic_header(DFL_EOB + 1, 1, w.codegens(), false);
+            if (w.nbits) w.byte((uint8_t)w.bits);
+            for (uint64_t j = w.n; j < sizeof(r->hbits); j++) r->hbits[j] = 0;
+        }
+    }
+    __syncthreads();
+    if (r->est >= 0)
+        for (uint32_t t = tid; t <= DFL_EOB; t += DFL_NOLZ_THREADS) r->codes[t] = st->lit[0].codes[t];
+}
+
+// plan, level -2: writeBlockHuff's decisions for the windows of an input of n bytes, in order, on one warp.  Lane l holds
+// the table in force's codes for bytes 8l .. 8l + 7; the next window's fields are loaded while this one is decided.
+B2C_DEV void dfl_nolz_walk(DflNolzWin *R, uint32_t nw, uint32_t n, unsigned lane) {
+    int L = 0;                                         // lastHeader
+    uint32_t t = 0, teob = 0, tc[8];                   // the table in force: its window, EOB code, this lane's codes
+    for (int j = 0; j < 8; j++) tc[j] = 0;
+    uint64_t p = 0;
+    int nest = R[0].est, nhdr = R[0].hdr;
+    uint4 nh = reinterpret_cast<const uint4 *>(R[0].hist)[lane];
+    for (uint32_t k = 0; k < nw; k++) {
+        DflNolzWin *r = R + k;
+        const int est0 = nest, hdr = nhdr;
+        const uint4 h = nh;
+        if (k + 1 < nw) { nest = R[k + 1].est; nhdr = R[k + 1].hdr; nh = reinterpret_cast<const uint4 *>(R[k + 1].hist)[lane]; }
+        const uint32_t len = k + 1 < nw ? DFL_NOLZ_WINDOW_HUFF : n - k * DFL_NOLZ_WINDOW_HUFF;
+        const bool sync = k + 1 == nw;
+        bool stored = est0 < 0;
+        int est = 0;
+        if (!stored) {
+            est = est0 + (L ? L : 70 * 8);
+            est += est >> DFL_NOLZ_PEN;
+            stored = (int)(len + 5) * 8 <= est;
+        }
+        uint32_t eob = 0, use = DFL_NOLZ_STORED;
+        uint64_t bits;
+        if (stored) {                                  // writeStoredHeader: the owed EOB, 3 bits, the byte's end, LEN/NLEN
+            if (L > 0) eob = teob;
+            L = 0;
+            bits = (((p + (eob & 0xff) + 3 + 7) & ~7ull) - p) + 32 + 8 * (uint64_t)len;
+        } else {
+            int reuse = 0x7fffffff;
+            if (L > 0) {                               // canReuseBits(table in force, literalFreq[:256])
+                const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
+                int part = 0;
+                bool miss = false;
+                for (int j = 0; j < 8; j++) {
+                    const uint32_t f = (hw[j >> 1] >> (16 * (j & 1))) & 0xffff;
+                    if (f) { miss = miss || tc[j] == 0; part += (int)f * (int)(tc[j] & 0xff); }
+                }
+                for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(FULLMASK, part, o);
+                reuse = __any_sync(FULLMASK, miss) ? 0x7fffffff : part;
+                if (est < reuse) { eob = teob; L = 0; }
+            }
+            if (L == 0) {                              // a new table: this window's
+                t = k; L = hdr;
+                const uint4 a = reinterpret_cast<const uint4 *>(r->codes)[2 * lane],
+                            b = reinterpret_cast<const uint4 *>(r->codes)[2 * lane + 1];
+                tc[0] = a.x; tc[1] = a.y; tc[2] = a.z; tc[3] = a.w; tc[4] = b.x; tc[5] = b.y; tc[6] = b.z; tc[7] = b.w;
+                teob = r->codes[DFL_EOB];
+                bits = (uint64_t)hdr + est0 - (teob & 0xff);
+            } else {
+                bits = (uint64_t)reuse;
+            }
+            use = t;
+            bits += eob & 0xff;
+            if (sync) { bits += teob & 0xff; L = 0; }
+        }
+        if (lane == 0) { r->bit = p; r->end = p + bits; r->eob = eob; r->use = use; r->sync = sync; }
+        p += bits;
+    }
+}
+
+// plan: one warp per input of the pass.  The member's size, B2C_ERR_DST_SMALL if it does not fit (nothing is written),
+// else the header, the close block's bytes after the one a window shares, the trailer and the checksum.
+B2C_DEV void dfl_nolz_plan_warp(const DflNolzParams &P, uint32_t i, unsigned lane) {
+    if (dfl_nolz_refused(P, i)) { if (lane == 0) P.out_sizes[i] = DFL_ERR_ARG; return; }
+    const uint32_t n = P.src_sizes[i], nw = dfl_nolz_windows(n, P.level);
+    DflNolzWin *R = P.wins + (uint64_t)(i - P.i0) * P.max_windows;
+    uint32_t acc[2] = {0, 0};
+    if (dfl_nolz_checked(P)) {
+        for (uint32_t k = lane; k < nw; k += 32) dfl_nolz_check_add(P, acc, R[k].check);
+        for (int o = 16; o; o >>= 1) {
+            const uint32_t t[2] = {__shfl_xor_sync(FULLMASK, acc[0], o), __shfl_xor_sync(FULLMASK, acc[1], o)};
+            dfl_nolz_check_add(P, acc, t);
+        }
+    }
+    const uint32_t check = P.format == DFL_FMT_ZLIB ? ((acc[1] + n % DFL_ADLER_MOD) % DFL_ADLER_MOD) << 16 | (acc[0] + 1) % DFL_ADLER_MOD
+                                                     : acc[0];
+    uint64_t sc;                                       // the close block's first bit
+    if (P.level == 0) {                                // every window stored: len + 5 bytes, byte-aligned
+        for (uint32_t k = lane; k < nw; k += 32) {
+            const uint32_t len = k + 1 < nw ? DFL_NOLZ_WINDOW_STORE : n - k * DFL_NOLZ_WINDOW_STORE;
+            DflNolzWin *r = R + k;
+            r->bit = (uint64_t)k * (DFL_NOLZ_WINDOW_STORE + 5) * 8; r->end = r->bit + (uint64_t)(len + 5) * 8;
+            r->eob = 0; r->use = DFL_NOLZ_STORED; r->sync = k + 1 == nw;
+        }
+        sc = (uint64_t)n + 5ull * nw;
+        sc *= 8;
+    } else {
+        if (nw) dfl_nolz_walk(R, nw, n, lane);
+        __syncwarp();
+        sc = nw ? R[nw - 1].end : 0;
+    }
+    const uint32_t hoff = dfl_nolz_hoff(P), tl = P.format == DFL_FMT_GZIP ? 8 : (P.format == DFL_FMT_ZLIB ? 4 : 0);
+    const uint64_t cend = (sc + 10 + 7) >> 3, total = hoff + cend + tl;
+    if (total > (P.dst_caps ? P.dst_caps[i] : P.dst_cap)) { if (lane == 0) P.out_sizes[i] = -4; return; }
+    uint8_t *o = dfl_nolz_dst(P, i);
+    if (P.format == DFL_FMT_ZLIB) { if (lane < 2) o[lane] = lane ? 0x01 : 0x78; }   // zlib/writer.go:95-130 at -2 / 0
+    else for (uint32_t k = lane; k < hoff; k += 32) o[k] = P.hdr[k];
+    // writeStoredHeader(0, true): the fixed header 011 then 7 zero bits, then the byte's end.  Its first byte is a
+    // window's last when the block does not start a byte (the finish pass writes that one).
+    const uint64_t c0 = sc >> 3;
+    const uint32_t cb = 3u << (sc & 7);
+    for (uint64_t b = c0 + ((sc & 7) ? 1 : 0) + lane; b < cend; b += 32) o[hoff + b] = (uint8_t)(cb >> (8 * (b - c0)));
+    uint8_t *tr = o + hoff + cend;
+    if (lane < 4) {
+        if (P.format == DFL_FMT_GZIP) { tr[lane] = (uint8_t)(check >> (8 * lane)); tr[4 + lane] = (uint8_t)(n >> (8 * lane)); }
+        else if (P.format == DFL_FMT_ZLIB) tr[lane] = (uint8_t)(check >> (24 - 8 * lane));
+    }
+    if (lane == 0) {
+        if (P.crc_out) P.crc_out[i] = check;
+        P.out_sizes[i] = (int64_t)total;
+    }
+}
+
+// `nb` bits of v at bit `pos` of the staging words (v < 2^nb, nb <= 32)
+B2C_DEV void dfl_nolz_or(uint32_t *stage, uint64_t pos, uint32_t v, uint32_t nb) {
+    const uint32_t w = (uint32_t)(pos >> 5), sh = (uint32_t)(pos & 31);
+    if (v == 0) return;
+    atomicOr(&stage[w], v << sh);
+    if (sh && sh + nb > 32) atomicOr(&stage[w + 1], v >> (32 - sh));
+}
+
+// emit: one CTA of DFL_NOLZ_THREADS per window slot g.  Shared: stage[DFL_NOLZ_STAGE_WORDS], codes[257],
+// wsum[DFL_NOLZ_THREADS / 32].  The window's bits are ORed into the staging words at their offsets from the byte its
+// range starts in, then the bytes the range covers whole go out; its partial first and last bytes go to its record.
+B2C_DEV void dfl_nolz_emit(const DflNolzParams &P, uint64_t g, uint32_t *stage, uint32_t *codes, uint32_t *wsum,
+                           unsigned tid) {
+    DflNolzSlot s;
+    if (!dfl_nolz_slot(P, g, s) || P.out_sizes[s.i] < 0) return;
+    DflNolzWin *r = P.wins + g;
+    const uint32_t W = dfl_nolz_window(P.level), ws = s.k * W, len = s.n - ws < W ? s.n - ws : W;
+    const uint8_t *in = dfl_nolz_src(P, s.i) + ws;
+    const uint64_t bit = r->bit, end = r->end, b0 = bit >> 3;
+    const uint32_t rb = (uint32_t)(bit & 7), eob = r->eob, use = r->use, el = eob & 0xff;
+    uint8_t *out = dfl_nolz_dst(P, s.i) + dfl_nolz_hoff(P) + b0;
+    const uint8_t *sb = reinterpret_cast<const uint8_t *>(stage);
+    if (use == DFL_NOLZ_STORED) {                      // the owed EOB, 3 zero bits, the byte's end, LEN / NLEN, the bytes
+        const uint32_t pos = ((rb + el + 3 + 7) & ~7u) + 32;
+        const uint64_t v = (uint64_t)(eob >> 8) << rb | (uint64_t)len << (pos - 32) | (uint64_t)(uint16_t)~len << (pos - 16);
+        for (uint32_t j = (rb ? 1 : 0) + tid; j < pos / 8; j += DFL_NOLZ_THREADS) out[j] = (uint8_t)(v >> (8 * j));
+        for (uint32_t j = tid; j < len; j += DFL_NOLZ_THREADS) out[pos / 8 + j] = in[j];
+        if (tid == 0) r->pieces = rb ? (uint32_t)(v & 0xff) : 0;
+        return;
+    }
+    const uint32_t nwords = (uint32_t)((end - 8 * b0 + 31) >> 5);
+    for (uint32_t j = tid; j < nwords; j += DFL_NOLZ_THREADS) stage[j] = 0;
+    const DflNolzWin *tr = P.wins + (g - s.k) + use;
+    for (uint32_t j = tid; j <= DFL_EOB; j += DFL_NOLZ_THREADS) codes[j] = tr->codes[j];
+    __syncthreads();
+    uint64_t pos = rb;
+    if (tid == 0) dfl_nolz_or(stage, pos, eob >> 8, el);
+    pos += el;
+    if (use == s.k) {                                  // a new table: its dynamic header
+        const uint32_t hb = (uint32_t)r->hdr;
+        const uint32_t *hw = reinterpret_cast<const uint32_t *>(r->hbits);
+        for (uint32_t j = tid; j * 32 < hb; j += DFL_NOLZ_THREADS)
+            dfl_nolz_or(stage, pos + 32 * j, hw[j], hb - 32 * j < 32 ? hb - 32 * j : 32);
+        pos += hb;
+    }
+    // the symbols: thread t codes the bytes [t * C, (t + 1) * C), placed by a block-wide scan of their code lengths
+    const uint32_t C = (len + DFL_NOLZ_THREADS - 1) / DFL_NOLZ_THREADS;
+    const uint32_t lo = tid * C < len ? tid * C : len, hi = lo + C < len ? lo + C : len;
+    uint32_t mine = 0;
+    for (uint32_t j = lo; j < hi; j++) mine += codes[in[j]] & 0xff;
+    uint32_t incl = mine;
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t v = __shfl_up_sync(FULLMASK, incl, o);
+        if ((tid & 31) >= (unsigned)o) incl += v;
+    }
+    if ((tid & 31) == 31) wsum[tid >> 5] = incl;
+    __syncthreads();
+    uint64_t at = pos + incl - mine;
+    for (uint32_t w = 0; w < (tid >> 5); w++) at += wsum[w];
+    uint64_t acc = 0;
+    uint32_t na = 0;
+    for (uint32_t j = lo; j < hi; j++) {
+        const uint32_t c = codes[in[j]];
+        acc |= (uint64_t)(c >> 8) << na;
+        na += c & 0xff;
+        if (na >= 32) { dfl_nolz_or(stage, at, (uint32_t)acc, 32); at += 32; acc >>= 32; na -= 32; }
+    }
+    if (na) dfl_nolz_or(stage, at, (uint32_t)acc, na);
+    if (tid == DFL_NOLZ_THREADS - 1 && r->sync) dfl_nolz_or(stage, at + na, codes[DFL_EOB] >> 8, codes[DFL_EOB] & 0xff);
+    __syncthreads();
+    const uint64_t last = (end >> 3) - b0;             // the byte the range ends in, partial when end is not aligned
+    for (uint64_t j = (rb ? 1 : 0) + tid; j < last; j += DFL_NOLZ_THREADS) out[j] = sb[j];
+    if (tid == 0) r->pieces = (rb ? sb[0] : 0u) | ((end & 7) ? (uint32_t)sb[last] << 8 : 0u);
+}
+
+// finish (level -2): thread for window slot g.  The byte its range ends in, when the range does not end a byte and starts
+// at or before the byte's first bit: its last piece, the first pieces of the windows that start in the byte, and the
+// close block's first bits when it starts there too.
+B2C_DEV void dfl_nolz_finish(const DflNolzParams &P, uint64_t g) {
+    DflNolzSlot s;
+    if (!dfl_nolz_slot(P, g, s) || P.out_sizes[s.i] < 0) return;
+    const DflNolzWin *R = P.wins + (g - s.k), *r = R + s.k;
+    const uint64_t end = r->end, B = end >> 3;
+    if ((end & 7) == 0 || r->bit > 8 * B) return;
+    uint32_t v = r->pieces >> 8;
+    uint32_t j = s.k + 1;
+    for (; j < s.nw && R[j].bit < 8 * B + 8; j++) v |= R[j].pieces & 0xff;
+    if (j == s.nw) {
+        const uint64_t sc = R[s.nw - 1].end;
+        if (sc < 8 * B + 8) v |= (3u << (sc & 7)) & 0xff;
+    }
+    dfl_nolz_dst(P, s.i)[dfl_nolz_hoff(P) + B] = (uint8_t)v;
+}
+
 #ifndef B2C_EMU
 constexpr int DFL_PARSE_WARPS = 2, DFL_ENCODE_LANES = 64, DFL_CRC_WARPS = 4;
 extern "C" __global__ void __launch_bounds__(DFL_PARSE_WARPS * 32) b2c_deflate_parse_kernel(DflParams P, uint32_t nchunks) {
@@ -892,6 +1277,27 @@ extern "C" __global__ void __launch_bounds__(DFL_CRC_WARPS * 32) b2c_deflate_l1_
     __syncthreads();
     const uint32_t i = blockIdx.x * DFL_CRC_WARPS + (threadIdx.x >> 5);
     if (i < nchunks) dfl_l1_check_warp(P, i, tab, threadIdx.x & 31);
+}
+// HuffmanOnly / NoCompression: block g of analysis and emit takes window slot g of the pass; plan: warp w takes input
+// i0 + w; finish: thread g takes slot g
+constexpr int DFL_NOLZ_PLAN_WARPS = 4;
+extern "C" __global__ void __launch_bounds__(DFL_NOLZ_THREADS) b2c_deflate_nolz_analyse_kernel(DflNolzParams P) {
+    __shared__ DflState st;
+    __shared__ uint32_t hist[256], terms[2 * DFL_NOLZ_THREADS / 32], tab[256];
+    inf_crc_table(tab, threadIdx.x, blockDim.x);
+    dfl_nolz_analyse(P, blockIdx.x, &st, hist, terms, tab, threadIdx.x);
+}
+extern "C" __global__ void __launch_bounds__(DFL_NOLZ_PLAN_WARPS * 32) b2c_deflate_nolz_plan_kernel(DflNolzParams P) {
+    const uint32_t i = P.i0 + blockIdx.x * DFL_NOLZ_PLAN_WARPS + (threadIdx.x >> 5);
+    if (i < P.i1) dfl_nolz_plan_warp(P, i, threadIdx.x & 31);
+}
+extern "C" __global__ void __launch_bounds__(DFL_NOLZ_THREADS) b2c_deflate_nolz_emit_kernel(DflNolzParams P) {
+    __shared__ uint32_t stage[DFL_NOLZ_STAGE_WORDS], codes[DFL_EOB + 1], wsum[DFL_NOLZ_THREADS / 32];
+    dfl_nolz_emit(P, blockIdx.x, stage, codes, wsum, threadIdx.x);
+}
+extern "C" __global__ void __launch_bounds__(DFL_NOLZ_THREADS) b2c_deflate_nolz_finish_kernel(DflNolzParams P, uint64_t slots) {
+    const uint64_t g = (uint64_t)blockIdx.x * DFL_NOLZ_THREADS + threadIdx.x;
+    if (g < slots) dfl_nolz_finish(P, g);
 }
 #endif
 

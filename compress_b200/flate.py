@@ -9,6 +9,12 @@ Encoder.best_speed_chunks / best_speed_device write what flate.NewWriter(w, Best
 .NewWriterLevel(w, BestSpeed) -- writes for Writes then Close, byte-identical to the reference: one lane per input parses
 and writes its windows in order.  NewWriter(w, BestSpeed) buffers its Writes and makes one such call at Close.
 
+Encoder.nolz_chunks / nolz_device write what the reference's writers write at HuffmanOnly (-2) and NoCompression (0):
+neither level has a match finder, so every window of every input is analysed and written in parallel, and a single
+large member is the whole device's work.  These methods are the way to raw and zlib streams at these levels: NewWriter
+here and zlib.NewWriterLevel keep raising ValueError for them.  gzip.NewWriterLevel(w, HuffmanOnly | NoCompression)
+buffers its Writes and makes one such call at Close.
+
 Decoder.decode_chunks / decode_device decode a batch of whole streams in one call, one lane per stream; results are the
 content's bytes or the reference's error class (B2C_ERR_* codes, see include/b2c.h).  NewReader and the readers of the gzip
 and zlib modules are thin layers over one such call for a single input: a single stream is serial, so one long stream
@@ -30,6 +36,9 @@ MAX_CAP = (1 << 32) - 1                      # contents are under 4 GiB
 MAX_STATELESS_DICT = 8 << 10                 # only the last 8 KiB of a dict are used
 BestSpeed = 1
 MAX_BEST_SPEED_INPUT = 1 << 30               # a larger input is B2C_ERR_ARG
+NoCompression, HuffmanOnly = 0, -2
+ConstantCompression = HuffmanOnly
+MAX_NOLZ_INPUT = (1 << 32) - 1               # inputs are under 4 GiB at HuffmanOnly / NoCompression
 
 
 class CorruptInputError(Exception):
@@ -226,6 +235,52 @@ class Encoder(Context):
         return (*t.results(), [int(c) for c in chk])
 
 
+    def nolz_device(self, level, src, src_sizes, src_stride, dst=None, dst_cap=None, out_sizes=None, format=RAW,
+                    header=b"", check_out=None, src_offsets=None):
+        """Device-resident batch at `level` (HuffmanOnly or NoCompression): input i is src_sizes[i] bytes at src + i *
+        src_stride (or src + src_offsets[i], each at most src_stride bytes), written as one member of `format` (RAW, ZLIB,
+        or GZIP with this member header) into row i of dst ([n, dst_cap] uint8).  check_out: optional int32 tensor for
+        each input's CRC-32 (RAW, GZIP) or Adler-32 (ZLIB).  Asynchronous on the current stream.  Returns (dst,
+        out_sizes): out_sizes[i] = bytes or a negative B2C_ERR_* code."""
+        assert src.is_cuda and src.dtype == torch.uint8
+        n = src_sizes.numel()
+        if dst_cap is None:
+            dst_cap = NoLZBound(level, src_stride) + _container_bytes(format, header)
+        if dst is None:
+            dst = torch.empty((n, dst_cap), dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty((n,), dtype=torch.int64, device=src.device)
+        stream = torch.cuda.current_stream(src.device).cuda_stream
+        check(lib.b2c_flate_nolz_device(self._ctx, level, format, 0, src.data_ptr(), src_stride,
+                                        None if src_offsets is None else src_offsets.data_ptr(), src_sizes.data_ptr(),
+                                        bytes(header), len(header), dst.data_ptr(),
+                                        dst.shape[1] if dst.dim() == 2 else dst_cap, None, dst_cap, out_sizes.data_ptr(),
+                                        None if check_out is None else check_out.data_ptr(), n, ctypes.c_void_p(stream)),
+              self._ctx)
+        return dst, out_sizes
+
+    def nolz_chunks(self, level, inputs, format=RAW, header=b"", caps=None):
+        """Host buffers at `level` (HuffmanOnly or NoCompression): one member of `format` per input.  Returns (outputs,
+        codes, checks): outputs[i] the bytes (None on error), codes[i] their length or a negative B2C_ERR_* code,
+        checks[i] the CRC-32 (RAW, GZIP) or Adler-32 (ZLIB) of input i."""
+        n = len(inputs)
+        if n == 0:
+            return [], [], []
+        if caps is None:
+            caps = [NoLZBound(level, len(b)) + _container_bytes(format, header) for b in inputs]
+        t = PointerTable(inputs, caps)
+        chk = (ctypes.c_uint32 * n)()
+        check(lib.b2c_flate_nolz_chunks(self._ctx, level, format, 0, t.srcs, t.ssz, bytes(header), len(header), t.dsts,
+                                        t.dcap, t.res, chk, n), self._ctx)
+        return (*t.results(), [int(c) for c in chk])
+
+
+def NoLZBound(level, n):
+    """The largest raw output of an n-byte input at HuffmanOnly or NoCompression (a zlib stream adds 6 bytes, a gzip
+    member its header + 8); 0 for another level."""
+    return int(lib.b2c_flate_nolz_bound(level, n))
+
+
 def BestSpeedBound(n):
     """The largest raw output of an n-byte input at BestSpeed (a zlib stream adds 6 bytes, a gzip member its header + 8)."""
     return int(lib.b2c_flate_best_speed_bound(n))
@@ -339,6 +394,16 @@ class Writer(BufferedWriter):
         return best_speed_member(data, RAW)
 
 
+def nolz_member(data, level, format, header=b""):
+    """One member of `format` at HuffmanOnly or NoCompression for the bytes of all Writes, encoded in one device call;
+    raises on error."""
+    outs, codes, _ = _encoder().nolz_chunks(level, [data], format, header)
+    if codes[0] < 0:
+        raise B2CError(f"libb200comp error {codes[0]}: {lib.b2c_strerror(codes[0]).decode()}")
+    return outs[0]
+
+
 def NewWriter(w, level):
-    """flate.NewWriter; only BestSpeed is built."""
+    """flate.NewWriter; only BestSpeed is built.  Raw streams at HuffmanOnly and NoCompression come from
+    Encoder.nolz_chunks / nolz_device (this still raises ValueError for them)."""
     return Writer(w, level)

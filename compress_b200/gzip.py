@@ -2,8 +2,9 @@
 input is serial; see flate.Decoder for batches).  The first member's Header is parsed on the host.
 
 gzip.NewWriterLevel(w, StatelessCompression) (gzip/gzip.go): a Writer whose every Write is one device call of
-flate.StatelessDeflate; the CRC-32 is continued on the device.  gzip.NewWriterLevel(w, BestSpeed): a Writer that buffers its
-Writes and encodes the member in one device call at Close.  Other levels are not built."""
+flate.StatelessDeflate; the CRC-32 is continued on the device.  gzip.NewWriterLevel(w, BestSpeed | HuffmanOnly |
+NoCompression): a Writer that buffers its Writes and encodes the member in one device call at Close.  Other levels are not
+built."""
 import io
 import struct
 from dataclasses import dataclass
@@ -14,6 +15,10 @@ from .flate import ErrUnexpectedEOF  # noqa: F401
 
 StatelessCompression = -3
 BestSpeed, BestCompression = 1, 9
+NoCompression, HuffmanOnly = 0, -2
+ConstantCompression = HuffmanOnly
+_BUFFERED = {BestSpeed: (flate.MAX_BEST_SPEED_INPUT, "1 GiB"), HuffmanOnly: (flate.MAX_NOLZ_INPUT, "4 GiB - 1"),
+             NoCompression: (flate.MAX_NOLZ_INPUT, "4 GiB - 1")}   # the levels whose member is one call at Close
 # time.Time{}.Unix(): the reference writes uint32(ModTime.Unix()) without a zero check, so an unset ModTime is this
 ZERO_MODTIME = -62135596800
 
@@ -101,17 +106,19 @@ def NewReader(r):
 
 
 class Writer:
-    """gzip.Writer at StatelessCompression or BestSpeed: Name / Comment / Extra / ModTime (Unix seconds; unset is Go's
-    zero time) / OS set before the first Write (at BestSpeed: before Close) go into the header.
+    """gzip.Writer at StatelessCompression, BestSpeed, HuffmanOnly or NoCompression: Name / Comment / Extra / ModTime
+    (Unix seconds; unset is Go's zero time) / OS set before the first Write (at the other levels: before Close) go into
+    the header.
     StatelessCompression: each Write(p) is StatelessDeflate(p, false), Close writes StatelessDeflate(nil, true), the
     CRC-32 and ISIZE; Flush writes nothing (the stateless writer keeps no pending data).
-    BestSpeed: the Writes are buffered and Close writes the whole member (header with XFL 4, the stream, CRC-32 and ISIZE)
-    from one device call; Flush (a sync flush) is not built and raises."""
+    BestSpeed, HuffmanOnly, NoCompression: the Writes are buffered and Close writes the whole member (header with XFL 4
+    at BestSpeed, else 0, the stream, CRC-32 and ISIZE) from one device call; Flush (a sync flush) is not built and
+    raises."""
 
     def __init__(self, w, level=StatelessCompression):
-        if level not in (StatelessCompression, BestSpeed):
-            raise ValueError("gzip: only StatelessCompression (-3) and BestSpeed (1) are built on the device; level %r is "
-                             "not" % (level,))
+        if level != StatelessCompression and level not in _BUFFERED:
+            raise ValueError("gzip: only StatelessCompression (-3), HuffmanOnly (-2), NoCompression (0) and BestSpeed (1) "
+                             "are built on the device; level %r is not" % (level,))
         self._level = level
         self.Reset(w)
 
@@ -135,11 +142,12 @@ class Writer:
 
     def Write(self, p):
         p = bytes(p)
-        if self._level == BestSpeed:
+        if self._level in _BUFFERED:
             if self._closed:
                 raise ValueError("write after Close")
-            if len(self._buf) + len(p) > flate.MAX_BEST_SPEED_INPUT:
-                raise ValueError("the device encodes at most 1 GiB per member at BestSpeed")
+            limit, text = _BUFFERED[self._level]
+            if len(self._buf) + len(p) > limit:
+                raise ValueError("the device encodes at most %s per member at level %d" % (text, self._level))
             self._buf += p
             return len(p)
         if not self._wrote:
@@ -156,15 +164,20 @@ class Writer:
     write = Write
 
     def Flush(self):
-        if self._level == BestSpeed:
-            raise NotImplementedError("Flush (a sync flush) is not built on the device at BestSpeed; Close ends the member")
+        if self._level in _BUFFERED:
+            raise NotImplementedError("Flush (a sync flush) is not built on the device at level %d; Close ends the member"
+                                      % self._level)
 
     def Close(self):
         if self._closed:
             return
         self._closed = True
-        if self._level == BestSpeed:
-            self._w.write(flate.best_speed_member(bytes(self._buf), flate.GZIP, self._header()))
+        if self._level in _BUFFERED:
+            data = bytes(self._buf)
+            if self._level == BestSpeed:
+                self._w.write(flate.best_speed_member(data, flate.GZIP, self._header()))
+            else:
+                self._w.write(flate.nolz_member(data, self._level, flate.GZIP, self._header()))
             self._buf = bytearray()
             return
         if not self._wrote:
@@ -175,7 +188,7 @@ class Writer:
 
 
 def NewWriterLevel(w, level):
-    """gzip.NewWriterLevel; only StatelessCompression and BestSpeed are built."""
+    """gzip.NewWriterLevel; only StatelessCompression, HuffmanOnly, NoCompression and BestSpeed are built."""
     return Writer(w, level)
 
 

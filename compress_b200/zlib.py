@@ -2,7 +2,9 @@
 (a single stream is serial; see flate.Decoder for batches).
 
 zlib.NewWriterLevel(w, BestSpeed) (zlib/writer.go): a Writer that buffers its Writes and encodes the stream in one device
-call at Close.  Other levels, and so NewWriter's DefaultCompression, are not built."""
+call at Close.  Other levels, and so NewWriter's DefaultCompression, are not built.  zlib streams at HuffmanOnly and
+NoCompression come from flate.Encoder.nolz_chunks / nolz_device with format ZLIB; NewWriterLevel raises ValueError for
+them."""
 import io
 
 from . import flate
@@ -49,5 +51,6 @@ def NewWriter(w):
 
 
 def NewWriterLevel(w, level):
-    """zlib.NewWriterLevel; only BestSpeed is built."""
+    """zlib.NewWriterLevel; only BestSpeed is built (HuffmanOnly and NoCompression: flate.Encoder.nolz_chunks /
+    nolz_device)."""
     return Writer(w, level)

@@ -320,6 +320,32 @@ B2C_API int b2c_flate_best_speed_chunks(b2c_ctx *ctx, int format, int flags, con
                                         const size_t *dst_caps, int64_t *sizes_out, uint32_t *check_out, size_t n);
 
 /*
+ * DEFLATE at HuffmanOnly (-2, also ConstantCompression) and NoCompression (0), byte-identical to the reference on amd64:
+ * input i is one member of the given format as the reference's writers at `level` write it for any number of Write(p)
+ * calls (together, input i) followed by Close() -- B2C_FLATE_RAW flate.NewWriter(w, level); B2C_FLATE_ZLIB
+ * zlib.NewWriterLevel(w, level): header 78 01, the stream, Adler-32 big-endian; B2C_FLATE_GZIP gzip.NewWriterLevel(w,
+ * level): hdr (the member header, >= 10 bytes, XFL 0, built by the caller), the stream, CRC-32 and ISIZE.  Without Flush
+ * the blocks depend on the byte count alone (one block per 32 768-byte window at -2, per 65 535-byte window at 0), so the
+ * Writes' boundaries do not matter.  Neither level has a match finder, so every window of every input is analysed and
+ * written in parallel; only the -2 table-reuse decisions are walked in order, one warp per input.  A single large input
+ * is therefore the whole device's work.  Results: the member's bytes, or B2C_ERR_DST_SMALL (nothing is written), or
+ * B2C_ERR_ARG for an input over src_stride in the _device call; the other inputs are unaffected.  Inputs are under 4 GiB.
+ * d_check_out / check_out (optional) receive each input's CRC-32 (raw, gzip) or Adler-32 (zlib).  Any level other than -2
+ * and 0 is B2C_ERR_ARG.  The context holds a 1 840-byte record per window slot (max_windows per input, from src_stride or
+ * the largest input), at most 4 GiB (larger batches run in passes over whole inputs).  b2c_flate_nolz_bound(level, n):
+ * the largest raw output of an n-byte input (add 6 for zlib, hlen + 8 for gzip; 0 for another level).  Argument
+ * conventions as b2c_flate_best_speed_device / _chunks; flags is 0.
+ */
+B2C_API size_t b2c_flate_nolz_bound(int level, size_t n);
+B2C_API int b2c_flate_nolz_device(b2c_ctx *ctx, int level, int format, int flags, const void *d_src, size_t src_stride,
+                                  const uint64_t *d_src_offsets, const uint32_t *d_src_sizes, const void *hdr, size_t hlen,
+                                  void *d_dst, size_t dst_stride, const uint64_t *d_dst_offsets, uint32_t dst_cap,
+                                  int64_t *d_out_sizes, uint32_t *d_check_out, uint32_t nchunks, void *stream);
+B2C_API int b2c_flate_nolz_chunks(b2c_ctx *ctx, int level, int format, int flags, const void *const *srcs,
+                                  const size_t *src_sizes, const void *hdr, size_t hlen, void *const *dsts,
+                                  const size_t *dst_caps, int64_t *sizes_out, uint32_t *check_out, size_t n);
+
+/*
  * S2 / Snappy STREAMS (the framing format: s2.Writer.EncodeBuffer, s2/writer.go:357-470, and s2.Reader over a buffer,
  * s2/reader.go:249-420; constants and the masked CRC32-C: s2/s2.go:75-126).  A stream = the identifier chunk, then per
  * block (<= 64 KiB here, WriterBlockSize) one chunk: type (0 compressed, 1 uncompressed), 24-bit length, checksum of the

@@ -1,14 +1,16 @@
 #!/usr/bin/env python
-"""Device-resident StatelessDeflate and BestSpeed rates (input GB/s) and ratios on helpers.synth_text_torch text, raw and as
+"""Device-resident StatelessDeflate, BestSpeed, HuffmanOnly and NoCompression rates (input GB/s) and ratios on helpers.synth_text_torch text, raw and as
 gzip members (BestSpeed also as zlib streams), in two shapes: --gib of text as 64 KiB inputs and as 64 MiB inputs.  Each batch is encoded whole and timed with CUDA events
 (--warmup warm-ups, --steps steps, --big-steps for the 64 MiB shape; --shapes / --formats pick rows, so that the rows
 can be split across runs); the
-parse / encode / crc (BestSpeed: l1 / l1_check) kernels are timed with torch.profiler in a run of their own.  The device inflate of the raw output
+parse / encode / crc (BestSpeed: l1 / l1_check; HuffmanOnly / NoCompression: analyse / plan / emit / finish) kernels are timed with torch.profiler in a run of their own.  The device inflate of the raw output
 is timed in the same session, and zlib.compress at level 1 on every host core over the same inputs is a CPU line for
 context (it is zlib's level 1, not the reference's StatelessDeflate, which is Go and does not run here).  Records the card's
 name and power limit.  Prints one JSON line (and writes it to --out).
 usage: deflate_times.py [--gib G] [--warmup W] [--steps K] [--big-steps K] [--big-mib M] [--shapes small,big]
-       [--formats raw,zlib,gzip] [--levels stateless,best_speed] [--no-inflate] [--out FILE]"""
+       [--formats raw,zlib,gzip] [--levels stateless,best_speed,huffman_only,no_compression] [--no-inflate] [--out FILE]
+HuffmanOnly / NoCompression rows run with --big-mib 1024 as one 1 GiB input: those levels write every window of a member
+in parallel.  (One 1 GiB member at the other two levels is one lane's work, a minute or more per call.)"""
 import argparse
 import json
 import os
@@ -28,6 +30,9 @@ from compress_b200 import flate
 
 KERNELS = ["b2c_deflate_parse_kernel", "b2c_deflate_encode_kernel", "b2c_deflate_crc_kernel"]
 KERNELS_L1 = ["b2c_deflate_l1_kernel", "b2c_deflate_l1_check_kernel"]
+KERNELS_NOLZ = ["b2c_deflate_nolz_analyse_kernel", "b2c_deflate_nolz_plan_kernel", "b2c_deflate_nolz_emit_kernel",
+                "b2c_deflate_nolz_finish_kernel"]
+NOLZ_LEVELS = (("huffman_only", flate.HuffmanOnly), ("no_compression", flate.NoCompression))
 HDR = b"\x1f\x8b\x08\x00\x00\x00\x00\x00\x00\xff"
 HDR_L1 = b"\x1f\x8b\x08\x00\x00\x09\x6e\x88\x04\xff"    # XFL 4, as gzip.NewWriterLevel(w, BestSpeed) writes it
 
@@ -72,7 +77,7 @@ def main():
     ap.add_argument("--big-steps", type=int, default=20)
     ap.add_argument("--big-mib", type=int, default=64)
     ap.add_argument("--shapes", default="small,big", help="small: 64 KiB inputs, big: --big-mib inputs")
-    ap.add_argument("--formats", default="raw,zlib,gzip", help="zlib: BestSpeed rows only")
+    ap.add_argument("--formats", default="raw,zlib,gzip", help="zlib: not for stateless rows")
     ap.add_argument("--levels", default="stateless,best_speed")
     ap.add_argument("--no-inflate", action="store_true", help="skip the device inflate of the raw output")
     ap.add_argument("--out", default=None)
@@ -117,6 +122,24 @@ def main():
             res["rows"].append(row)
             print(json.dumps(row), flush=True)
         del dst
+        for lname, level in NOLZ_LEVELS:
+            if lname not in a.levels:
+                continue
+            cap = flate.NoLZBound(level, piece) + len(HDR) + 8
+            dst = torch.empty((n, cap), dtype=torch.uint8, device=dev)
+            for fmt, name, hdr in ((flate.RAW, "raw", b""), (flate.ZLIB, "zlib", b""), (flate.GZIP, "gzip", HDR)):
+                if name not in a.formats:
+                    continue
+                call = lambda: enc.nolz_device(level, src, sizes, piece, dst=dst, dst_cap=cap, out_sizes=out, format=fmt, header=hdr)  # noqa: E731
+                ms = timed(call, warm, steps)
+                o = out.cpu()
+                assert int(o.min()) > 0
+                row = {"shape": "%d x %d KiB" % (n, piece >> 10), "level": lname, "format": name, "ms": round(ms, 3),
+                       "input_GBps": round(total / ms / 1e6, 2), "ratio": round(total / int(o.sum()), 4), "steps": steps,
+                       "kernel_ms": kernel_ms(call, KERNELS_NOLZ)}
+                res["rows"].append(row)
+                print(json.dumps(row), flush=True)
+            del dst
         if "best_speed" not in a.levels:
             continue
         cap = flate.BestSpeedBound(piece) + len(HDR_L1) + 8
